@@ -27,6 +27,8 @@ Sources (numbers only; no reference source code is copied):
   threemir    /root/reference/src/rayoptics/codev/tests/threemir.seq (CODE V three-mirror
               compact: conic / aspheric mirrors, every surface decentered and tilted with
               'dec and return'), read by rayoptics_b200/seq.py
+  edge_sphere, edge_conic, edge_even, edge_radial, edge_stops
+              synthetic finite-conjugate lenses for the boundary rays of make_golden_edges.py
 """
 import importlib.util
 import os
@@ -357,6 +359,63 @@ def relay(pupil_key, pupil_value, name):
     return finish(M.OpticalModel(sm, osp, name=name), aim=False, apertures=True)
 
 
+EDGE_PROFILES = {
+    'sphere': lambda: M.Spherical(c=0.125),
+    'conic': lambda: M.Conic(c=0.125, cc=-0.5),
+    'even': lambda: M.EvenPolynomial(c=0.125, cc=-0.5, coefs=[0.0, 1e-4]),
+    'radial': lambda: M.RadialPolynomial(c=0.125, ec=0.5, coefs=[0.0, 0.0, 1e-4]),
+}
+
+
+def edge_lens(kind):
+    """Synthetic finite-conjugate lens for the boundary rays of make_golden_edges.py.  The object
+    sits in an index-2 medium, so surface 1 (the profile under test, index 2 -> 1.5, radius 8,
+    clear aperture 2) shows clipping, TIR (|sin I| > 3/4) and a miss (grazing at height ~8) to
+    rays parallel to the axis.  cv = 1/8 and the indices 2 and 1.5 are chosen so that the
+    quantities that decide (r**2 - L**2, n'**2 - n**2 sin**2 I, b**2 - a*c) cancel exactly for
+    some start rays instead of only approximately.  Surface 2 is a plano 1.5 -> 1.75 interface
+    that on-axis rays hit at its vertex."""
+    n2, n15, n175 = M.ConstantIndex(2.0, 'n2'), M.ConstantIndex(1.5, 'n15'), M.ConstantIndex(1.75, 'n175')
+    spec = [(M.Spherical(0.0), 'dummy', 10.0, n2, 1e3),
+            (EDGE_PROFILES[kind](), 'transmit', 6.0, n15, 2.0),
+            (M.Spherical(0.0), 'transmit', 5.0, n175, 20.0),
+            (M.Spherical(0.0), 'dummy', 0.0, None, 1e3)]
+    ifcs, gaps = [], []
+    for prf, mode, thi, med, ap in spec:
+        ifcs.append(M.Surface(profile=prf, interact_mode=mode, max_aperture=ap))
+        if med is not None:
+            gaps.append(M.Gap(thi, med))
+    wvls = [587.6]
+    sm = M.SequentialModel(ifcs, gaps, stop_surface=1, wvlns=wvls, ref_wvl=0)
+    fields = [M.Field(y=0.0), M.Field(x=0.3, y=0.5)]
+    osp = OpticalSpecs(WvlSpec(wvls, 0), PupilSpec(('object', 'epd'), 8.0),
+                       FieldSpec(('object', 'height'), 0.5, fields))
+    return finish(M.OpticalModel(sm, osp, name='edge_' + kind), aim=False, apertures=False)
+
+
+def edge_stops():
+    """Synthetic lens of plano interfaces with aperture lists (general kernel only): a
+    rectangular stop with an offset, then an offset circular stop (inside the rectangle) with an
+    offset circular obscuration.  Rays parallel to the axis keep their start x, y exactly up to
+    the stops."""
+    n15 = M.ConstantIndex(1.5, 'n15')
+    spec = [('dummy', 10.0, M.Air()), ('transmit', 3.0, n15), ('transmit', 4.0, M.Air()),
+            ('dummy', 0.0, None)]
+    ifcs, gaps = [], []
+    for mode, thi, med in spec:
+        ifcs.append(M.Surface(profile=M.Spherical(0.0), interact_mode=mode, max_aperture=1e3))
+        if med is not None:
+            gaps.append(M.Gap(thi, med))
+    ifcs[1].clear_apertures = [M.Rectangular(5.0, 4.0, x_offset=0.25, y_offset=-0.5)]
+    ifcs[2].clear_apertures = [M.Circular(3.0, x_offset=0.3, y_offset=0.2),
+                               M.Circular(1.0, is_obscuration=True, x_offset=-0.2, y_offset=0.1)]
+    wvls = [587.6]
+    sm = M.SequentialModel(ifcs, gaps, stop_surface=1, wvlns=wvls, ref_wvl=0)
+    osp = OpticalSpecs(WvlSpec(wvls, 0), PupilSpec(('object', 'epd'), 6.0),
+                       FieldSpec(('object', 'height'), 1.0, [M.Field(y=0.0), M.Field(y=1.0)]))
+    return finish(M.OpticalModel(sm, osp, name='edge_stops'), aim=False, apertures=False)
+
+
 def fisheye():
     import importlib
     import warnings
@@ -430,6 +489,8 @@ def main():
         'hybrid': lambda: from_roa('models/HybridAchromat.roa', 'hybrid'),
         'diffractive': diffractive,
         'diffractive_wild': diffractive_wild,
+        **{'edge_' + k: (lambda k=k: edge_lens(k)) for k in EDGE_PROFILES},
+        'edge_stops': edge_stops,
     }
     only = sys.argv[1:]
     for name, fn in models.items():

@@ -19,7 +19,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G = os.path.join(ROOT, 'tests', 'golden')
 GENERATORS = ('make_models.py', 'make_golden.py', 'make_golden_grids.py', 'make_golden_opd.py',
-              'make_golden_analyses.py')
+              'make_golden_analyses.py', 'make_golden_edges.py')
 
 
 def arrays(path):
