@@ -35,13 +35,14 @@
 extern "C" {
 #endif
 
-#define RT_ABI_VERSION 4
+#define RT_ABI_VERSION 5
 #define RT_MAX_COEFS 20     /* EvenPolynomial uses <=10, RadialPolynomial <=20 */
 #define RT_MAX_PHASE_COEFS 10
 #define RT_MAX_APERTURES 4  /* Surface.clear_apertures entries honoured per interface */
 #define RT_SEG_DOUBLES 10   /* one ray segment = p[3], d[3], dst, nrml[3]  (raytr/__init__.py:36) */
 #define RT_SUMMARY_DOUBLES 16
 #define RT_WAVE_DOUBLES 24   /* per-(field, wvl) chief-ray / reference-sphere record, see rt_grid_spec.wave */
+#define RT_MAX_FOCUS 64      /* image planes of one rt_trace_grid_focus call */
 
 /* error codes (function return values) */
 enum rt_error {
@@ -329,6 +330,31 @@ int rt_trace_grid_to_host(const rt_table *table, rt_grid *grid, int64_t chunk_be
  * or NULL, receives a copy. */
 int rt_grid_chief_ref(const rt_table *table, rt_grid *grid, int32_t wvl_idx,
                       double *ref_out, void *stream);
+
+/* ---- through focus (ABI 5): the spot sums of one grid trace at n_foc image planes.
+ * Plane k is evaluated with the epilogue of rt_trace_grid at foc = foc[k]: each ray's
+ * p + (foc[k]/d_z) d - ref_img[k][field].  Its summary row equals, column for column, the summary
+ * rt_trace_grid returns over the same chunk range for a grid with foc = foc[k] and the same
+ * reference points (both with the default dynamic schedule).  The through-focus trace always
+ * draws work items from a counter, so B200RT_STATIC does not apply to it. */
+/* chief-ray image intercepts defocused to every plane: ref_out[k][f] = p + (foc[k]/d_z) d of the
+ * ray rt_grid_chief_ref traces (calculate_reference_sphere's image_pt, raytr/waveabr.py:24-76).
+ * foc: HOST [n_foc]; ref_out: DEVICE [n_foc][n_fields][2].  The grid's own reference points are
+ * not changed.  One launch on `stream`. */
+int rt_grid_chief_ref_focus(const rt_table *table, const rt_grid *grid, int32_t wvl_idx,
+                            const double *foc, int32_t n_foc, double *ref_out, void *stream);
+/* DEVICE scratch bytes of rt_trace_grid_focus (n_foc times rt_grid_scratch_bytes); 0 for bad arguments */
+int64_t rt_grid_focus_scratch_bytes(const rt_grid *grid, int32_t n_foc,
+                                    int64_t chunk_begin, int64_t chunk_end);
+/* foc: HOST [n_foc], finite, 1 <= n_foc <= RT_MAX_FOCUS; ref_img: DEVICE [n_foc][n_fields][2] or
+ * NULL (= 0); summary: DEVICE [n_foc][n_tiles][RT_SUMMARY_DOUBLES] (required).  out: per-ray
+ * results as rt_trace_grid (p, d, op, status, fail_surf, n_seg); abr_x/abr_y/opd/full/nx/ny/nz/dst
+ * must be NULL.  RT_ERR_INVALID before any device work for bad arguments.  Two kernel launches
+ * whatever n_foc is. */
+int rt_trace_grid_focus(const rt_table *table, const rt_grid *grid,
+                        int64_t chunk_begin, int64_t chunk_end, const rt_opts *opts,
+                        const double *foc, int32_t n_foc, const double *ref_img,
+                        const rt_out *out, double *summary, void *scratch, void *stream);
 
 /* Combine n_parts partial summaries (chunk ranges of one grid, or the ranks' rows of an
  * all-gather): parts DEVICE [n_parts][n_tiles][RT_SUMMARY_DOUBLES] -> out DEVICE

@@ -244,6 +244,77 @@ def spot_diagram(opt_model, num_rays=21, fields=None, wvls=None, foc=None, table
                        grid.first_ray_of_chunk(c0), grid.n_rays, io)
 
 
+class ThroughFocus:
+    """Result of ``through_focus``.
+
+    ``foc`` ``[K]``: the focus shifts of the image planes; ``summary``: the ``spot_statistics``
+    keys as ``[K, n_fields, n_wvls]`` arrays, combined over all ranks; ``ref_img``
+    ``[K, n_fields, 2]``: the chief-ray image points defocused to each plane (the reference
+    points of that plane's aberrations); ``best_index`` / ``best_foc`` ``[n_fields, n_wvls]``:
+    the sampled plane of least ``rms_radius`` (-1 / NaN where no ray reaches the image)."""
+
+    def __init__(self, foc, summary, ref_img, num_rays, n_fields, n_wvls):
+        self.foc, self.summary, self.ref_img = foc, summary, ref_img
+        self.num_rays, self.n_fields, self.n_wvls = num_rays, n_fields, n_wvls
+        self.best_index, self.best_foc = best_focus(foc, summary['rms_radius'], summary['n_ok'])
+
+
+def focus_planes(defocus, num_planes):
+    """The planes of a FocusRange: ``defocus.get_focus(fr)`` for ``fr`` in ``linspace(-1, 1,
+    num_planes)``.  A zero ``defocus_range`` would make every plane the same: ValueError."""
+    if defocus.defocus_range == 0:
+        raise ValueError('the model\'s defocus_range is 0: pass the focus shifts as foc=')
+    return np.array([defocus.get_focus(fr) for fr in np.linspace(-1.0, 1.0, int(num_planes))])
+
+
+def best_focus(foc, rms_radius, n_ok):
+    """``(best_index, best_foc)`` over axis 0 of ``rms_radius`` ``[K, ...]``: the first plane of
+    least RMS radius; -1 and NaN where no ray reaches the image (``n_ok`` is 0 on every plane)."""
+    foc = np.asarray(foc, dtype=np.float64)
+    rms = np.where(np.asarray(n_ok) > 0, np.asarray(rms_radius, dtype=np.float64), np.inf)
+    rms = np.where(np.isnan(rms), np.inf, rms)
+    idx = np.argmin(rms, axis=0)
+    none = ~np.isfinite(rms).any(axis=0)
+    idx = np.where(none, -1, idx)
+    return idx, np.where(none, np.nan, foc[np.maximum(idx, 0)])
+
+
+def through_focus(opt_model, num_rays=21, foc=None, num_planes=21, fields=None, wvls=None, table=None,
+                  device=0, shard=None, group=None, chunk_range=None, **kwargs):
+    """RMS spot size against focus for every field and wavelength, from one grid trace.
+
+    The spot grid of ``spot_diagram`` is traced once and each ray's transverse aberration is
+    evaluated at every focus shift of ``foc`` (default: ``focus_planes(osp.defocus,
+    num_planes)``), referred to the chief ray at the central wavelength defocused to that plane
+    (``calculate_reference_sphere``'s image point, raytr/waveabr.py:24-76).  Only the per-plane
+    spot sums leave the device.  ``shard=(rank, world)`` / ``group`` / ``chunk_range`` as
+    ``spot_diagram``: one all-gather of the ``[K*n_tiles, 16]`` sums whatever K is.  At most
+    ``RT_MAX_FOCUS`` planes per call."""
+    from .parallel import shard_chunks, gather_summaries
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    foc = focus_planes(osp.defocus, num_planes) if foc is None else E._focus_array(foc)
+    table = _table_for(opt_model, table, device)
+    fields = list(osp.field_of_view.fields if fields is None else fields)
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    dev = torch.device('cuda', table.device)
+    with torch.cuda.device(dev):
+        # the grid's own foc is not used by the through-focus trace
+        grid, spec = _reusable_grid(opt_model, table, num_rays, fields, wvls, osp.defocus.focus_shift)
+        ref_dev = grid.chief_ref_focus(table, table.wvl_index(sm.central_wavelength()), foc)
+        c0, c1 = (0, grid.n_chunks) if shard is None else shard_chunks(grid.n_chunks, *shard)
+        if chunk_range is not None:
+            c0, c1 = chunk_range
+        summ = E.trace_grid_focus(table, grid, foc, c0, c1, ref_img=ref_dev, **kwargs)
+        if shard is not None:
+            summ = gather_summaries(summ.reshape(-1, summ.shape[-1]), group)
+        tail = torch.cat([summ.reshape(-1), ref_dev.reshape(-1)]).cpu().numpy()     # one small copy; waits
+    k, nf, nw = len(foc), len(fields), len(wvls)
+    summ_host = tail[:summ.numel()].reshape(k*nf*nw, -1)
+    stats = {key: np.asarray(v).reshape(k, nf, nw) for key, v in E.spot_statistics(summ_host).items()}
+    ref = tail[summ.numel():].reshape(k, nf, 2).copy()
+    return ThroughFocus(foc, stats, ref, num_rays, nf, nw)
+
+
 # --------------------------------------------------------------------------
 # RayFan / RayList / RayGrid: the reference's analysis classes
 # (/root/reference/src/rayoptics/raytr/analyses.py:121-187,343-434,584-663) with

@@ -7,6 +7,7 @@
  *   k_trace_grid<FULL,SUMMARY,STAGE>  start rays generated on device from the
  *                               (field, wavelength, pupil i, j) index, optional
  *                               per-chunk spot sums
+ *   k_trace_grid[_lean]_focus   one trace, spot sums at up to RT_MAX_FOCUS image planes
  *   k_reduce_summary            fixed-order per-tile reduction of the chunk sums
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
@@ -312,19 +313,112 @@ __device__ __forceinline__ void warp_record_from_regs(bool have, int status, dou
     if (lane == 0) dst[RT_ACC] = 1.0;
 }
 
+/* ---- through-focus spot sums (rt_trace_grid_focus): every ray is traced once and its
+ * transverse aberration is evaluated at n image planes.  Plane k's records reduce to the
+ * summary a single-focus rt_trace_grid launch at foc[k] returns over the same chunk range:
+ *  - chunk slots (the regime that launch would take): warp_record_from_regs's record, its sums
+ *    with the same shuffle tree;
+ *  - otherwise the per-item sums of item_sums_store (same tree, same item order in the
+ *    reduction) plus one record per (tile, CTA, warp) holding the counts and the min / max,
+ *    whose result does not depend on the order the rays are added in.
+ * The per-thread shared-memory accumulators of the static schedule would need n x 15 doubles
+ * per thread, so this path always draws work items from a counter (B200RT_STATIC is ignored). */
+struct FocusPlanes {
+    const double *foc;          /* [n] focus shifts: the kernel's shared-memory copy of FocusList */
+    const double *ref;          /* DEVICE [n][n_fields][2] reference image points, or NULL (= 0) */
+    int64_t n_tiles, n_items;   /* tiles of the grid; work items of the launch (one plane) */
+    int32_t n, n_fields, chunk_slots, pad_;
+};
+struct FocusList { double v[RT_MAX_FOCUS]; };
+
+/* constant-offset reads of the parameter array (a dynamically indexed kernel parameter would
+ * be copied to local memory); blockDim.x >= RT_MAX_FOCUS */
+__device__ __forceinline__ void stage_focus(const FocusList &L, int n, double *s)
+{
+#pragma unroll
+    for (int k = 0; k < RT_MAX_FOCUS; k++)
+        if ((int)threadIdx.x == k && k < n) s[k] = L.v[k];
+    __syncthreads();
+}
+
+__device__ __forceinline__ void focus_item(const FocusPlanes &F, bool have, int status, const Vec3 &p,
+                                           const Vec3 &d, double op, int f, int64_t tile, int64_t lc,
+                                           int slice, unsigned long long item, bool chunk_slots, bool first,
+                                           int64_t sl, double *scratch, double *item_sums)
+{
+    const int lane = threadIdx.x & 31;
+    const bool ok = have && status == RT_RAY_OK;
+    const int ck = status == RT_RAY_OK ? 0 : (status <= RT_RAY_BLOCKED ? status : 4);
+    /* record column this lane writes: 10..13 min / max (lanes 0, 8, 16, 24), 0..4 the status
+     * counts (lanes 1..5, the same on every plane), 15 the valid flag (lane 6) */
+    double cnt = 0.0;
+#pragma unroll
+    for (int c = 0; c < 5; c++) {
+        const unsigned m = __ballot_sync(0xffffffffu, have && ck == c);
+        if (lane == c + 1) cnt = (double)__popc(m);
+    }
+    const int col = (lane & 7) == 0 ? 10 + (lane >> 3) : (lane >= 1 && lane <= 5) ? lane - 1 : (lane == 6 ? 15 : -1);
+    const int64_t rec = chunk_slots ? (tile*sl + lc)*RT_WARPS + slice
+                                    : (tile*sl + blockIdx.x)*RT_WARPS + (threadIdx.x >> 5);
+    const bool h16 = lane & 16, h8 = lane & 8;
+    for (int k = 0; k < F.n; k++) {
+        const double rx = F.ref ? F.ref[((int64_t)k*F.n_fields + f)*2 + 0] : 0.0;
+        const double ry = F.ref ? F.ref[((int64_t)k*F.n_fields + f)*2 + 1] : 0.0;
+        /* the single-focus epilogue of grid_chunk_loop with G.foc -> foc[k] */
+        const double dist = div_maybe_zero(F.foc[k], d.z);
+        const double ax = (p.x + dist*d.x) - rx;
+        const double ay = (p.y + dist*d.y) - ry;
+        /* min / max in 6 shuffles: lower half-warp keeps x, upper y; then lanes 0-7 min, 8-15 max */
+        const double v0 = ok ? ax : CUDART_INF, v1 = ok ? ax : -CUDART_INF;
+        const double v2 = ok ? ay : CUDART_INF, v3 = ok ? ay : -CUDART_INF;
+        const double a0 = fmin(h16 ? v2 : v0, __shfl_xor_sync(0xffffffffu, h16 ? v0 : v2, 16));
+        const double a1 = fmax(h16 ? v3 : v1, __shfl_xor_sync(0xffffffffu, h16 ? v1 : v3, 16));
+        double b = __shfl_xor_sync(0xffffffffu, h8 ? a0 : a1, 8);
+        b = h8 ? fmax(a1, b) : fmin(a0, b);
+#pragma unroll
+        for (int s = 4; s > 0; s >>= 1) {
+            const double y = __shfl_xor_sync(0xffffffffu, b, s);
+            b = h8 ? fmax(b, y) : fmin(b, y);
+        }
+        double *dst = scratch + ((int64_t)k*F.n_tiles*sl*RT_WARPS + rec)*RT_SUMMARY_DOUBLES;
+        double v = col >= 10 && col <= 13 ? b : (col == 15 ? 1.0 : cnt);
+        if (chunk_slots) {
+            /* the sums exactly as warp_record_from_regs forms them */
+            const double s6[RT_ITEM_SUMS] = {ax, ay, ax*ax, ay*ay, ax*ay, op};
+            const int scol[RT_ITEM_SUMS] = {5, 6, 7, 8, 9, 14};
+#pragma unroll
+            for (int j = 0; j < RT_ITEM_SUMS; j++) {
+                double x = ok ? s6[j] : 0.0;
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) x = x + __shfl_down_sync(0xffffffffu, x, off);
+                if (lane == 0) dst[scol[j]] = x;
+            }
+        } else {
+            item_sums_store(ok, ax, ay, op, item_sums + ((int64_t)k*F.n_items + item)*RT_ITEM_SUMS);
+            /* a warp's items come in increasing order, so it never returns to a tile it has left */
+            if (!first && col >= 0 && col != 15) {
+                const double o = dst[col];
+                v = (col == 10 || col == 12) ? fmin(o, v) : (col == 11 || col == 13) ? fmax(o, v) : o + v;
+            }
+        }
+        if (col >= 0) dst[col] = v;
+    }
+}
+
 /* chunk loop shared by the general and the lean grid kernels: start ray ->
  * trace -> per-ray results -> transverse aberration (focus_pupil_coords,
- * analyses.py:561-580) -> spot sums */
-template <bool SUMMARY, bool WAVE, typename TraceFn>
+ * analyses.py:561-580) -> spot sums.  FOCUS: the spot sums of the planes of *FP instead
+ * (needs SUMMARY == false and a work counter). */
+template <bool SUMMARY, bool WAVE, bool FOCUS = false, typename TraceFn>
 __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_begin, int64_t chunk_end,
                                                 const rt_out &out, double *scratch, double *acc,
                                                 unsigned long long *work_counter, double *item_sums,
-                                                TraceFn trace)
+                                                TraceFn trace, const FocusPlanes *FP = nullptr)
 {
     const int64_t tile0 = chunk_begin/G.chunks_per_tile;
     const int64_t ray0 = tile0*G.rays_per_tile + (chunk_begin - tile0*G.chunks_per_tile)*RT_BLOCK;
     const int64_t sl = G.chunks_per_tile < RT_MAX_GRID ? G.chunks_per_tile : RT_MAX_GRID;
-    const bool chunk_slots = G.chunks_per_tile <= (int64_t)gridDim.x;
+    const bool chunk_slots = FOCUS ? FP->chunk_slots != 0 : G.chunks_per_tile <= (int64_t)gridDim.x;
     int64_t cur_tile = -1;
     if (SUMMARY && !chunk_slots) acc_init(acc);
     const unsigned long long n_items = (unsigned long long)(chunk_end - chunk_begin)*RT_WARPS;
@@ -359,6 +453,7 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
         }
         int status = RT_RAY_OK;
         double ax = 0.0, ay = 0.0, op = 0.0;
+        Vec3 fp = {0.0, 0.0, 0.0}, fd = {0.0, 0.0, 0.0};     /* FOCUS: image point and direction */
         if (have) {
             const int f = (int)(tile/G.n_wvls);
             const int w = (int)(tile - (int64_t)f*G.n_wvls);
@@ -368,6 +463,7 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             trace(f, w, loc, k, R, d0);
             store_result(out, k, R);
             status = R.status; op = R.op;
+            if (FOCUS) { fp = R.p; fd = R.d; }
             if (WAVE)
                 out.opd[k] = (R.status == RT_RAY_OK)
                                  ? wave_opd(G.wave + tile*RT_WAVE_DOUBLES, R.p1, d0, R.pk, R.dk, R.p, R.d, R.op)
@@ -398,6 +494,12 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
         if (SUMMARY && !chunk_slots && work_counter)
             item_sums_store(have && status == RT_RAY_OK, ax, ay, op, item_sums + item*RT_ITEM_SUMS);
         if (SUMMARY && chunk_slots) warp_record_from_regs(have, status, ax, ay, op, scratch, tile, lc, sl, slice);
+        if (FOCUS) {
+            const bool first = tile != cur_tile;
+            cur_tile = tile;
+            focus_item(*FP, have, status, fp, fd, op, (int)(tile/G.n_wvls), tile, lc, slice, item, chunk_slots,
+                       first, sl, scratch, item_sums);
+        }
         if (!work_counter) c += gridDim.x;
     }
     if (SUMMARY && !chunk_slots && cur_tile >= 0) acc_flush(acc, scratch, cur_tile, blockIdx.x, sl);
@@ -423,6 +525,33 @@ k_trace_grid(const rt_surface_desc *__restrict__ g_surfs, const double *__restri
             const int wi = G.wvl_idx[w];
             trace_ray<FULL, WAVE>(tab, ntab + (int64_t)wi*n_ifc, g_wvl[wi], n_ifc, o, p0, d0, fw, R);
         });
+}
+
+/* through-focus instance of k_trace_grid (per-ray outputs of kind 0 only) */
+template <bool STAGE>
+__global__ void __launch_bounds__(RT_BLOCK)
+k_trace_grid_focus(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                   int n_ifc, int n_wvl, GridDev G, int64_t chunk_begin, int64_t chunk_end,
+                   rt_opts o, rt_out out, double *__restrict__ scratch, const double *__restrict__ g_wvl,
+                   int pupil_kind, unsigned long long *work_counter, double *item_sums,
+                   FocusPlanes P, FocusList foc)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    __shared__ double s_foc[RT_MAX_FOCUS];
+    const rt_surface_desc *tab;
+    const double *ntab;
+    stage_focus(foc, P.n, s_foc);
+    stage_table<STAGE>(g_surfs, g_n, n_ifc, n_wvl, smem, tab, ntab);
+    FocusPlanes F = P;
+    F.foc = s_foc;
+    grid_chunk_loop<false, false, true>(G, chunk_begin, chunk_end, out, scratch, nullptr, work_counter, item_sums,
+        [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0) {
+            Vec3 p0;
+            grid_start_ray<false>(G, pupil_kind, f, loc, p0, d0);
+            FullWriter fw = {nullptr, 0};
+            const int wi = G.wvl_idx[w];
+            trace_ray<false, false>(tab, ntab + (int64_t)wi*n_ifc, g_wvl[wi], n_ifc, o, p0, d0, fw, R);
+        }, &F);
 }
 
 /* ---- lean kernels: plan built in shared memory by the CTA (rt_lean.cuh) */
@@ -477,6 +606,33 @@ k_trace_grid_lean(const rt_surface_desc *__restrict__ g_surfs, const double *__r
             FullWriter fw = {OUT == 2 ? out.full + k : nullptr, out.full_stride};
             trace_ray_lean<OUT, WAVE, POLY>(ls, li + (int64_t)G.wvl_idx[w]*n_ifc, lp, g_surfs, n_ifc, o, p0, d0, fw, R);
         });
+}
+
+/* through-focus instance of k_trace_grid_lean (per-ray outputs of kind 0 only) */
+template <bool POLY>
+__global__ void __launch_bounds__(RT_BLOCK, POLY ? 2 : RT_LEAN_MIN_CTAS)
+k_trace_grid_lean_focus(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                        int n_ifc, int n_wvl, GridDev G, int64_t chunk_begin, int64_t chunk_end,
+                        rt_opts o, rt_out out, double *__restrict__ scratch, unsigned long long *work_counter,
+                        double *item_sums, FocusPlanes P, FocusList foc)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    __shared__ double s_foc[RT_MAX_FOCUS];
+    LeanSurf *ls = reinterpret_cast<LeanSurf *>(smem);
+    LeanIdx *li = reinterpret_cast<LeanIdx *>(ls + n_ifc);
+    LeanPoly *lp = reinterpret_cast<LeanPoly *>(li + (size_t)n_ifc*n_wvl);      /* POLY instances only */
+    build_plan(g_surfs, g_n, n_ifc, n_wvl, o, ls, li);
+    if (POLY) build_poly_plan(g_surfs, n_ifc, lp);
+    stage_focus(foc, P.n, s_foc);                /* its barrier also completes the plan */
+    FocusPlanes F = P;
+    F.foc = s_foc;
+    grid_chunk_loop<false, false, true>(G, chunk_begin, chunk_end, out, scratch, nullptr, work_counter, item_sums,
+        [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0) {
+            Vec3 p0;
+            grid_start_ray<true>(G, RT_PUPIL_EPD, f, loc, p0, d0);
+            FullWriter fw = {nullptr, 0};
+            trace_ray_lean<0, false, POLY>(ls, li + (int64_t)G.wvl_idx[w]*n_ifc, lp, g_surfs, n_ifc, o, p0, d0, fw, R);
+        }, &F);
 }
 
 /* division self-test: div_shared/normalize3_shared against the IEEE `/` */
@@ -548,16 +704,22 @@ __device__ __forceinline__ double red_op(int k, double a, double y)
     return a + y;
 }
 
-__global__ void __launch_bounds__(RT_RED_THREADS)
-k_reduce_summary(const double *__restrict__ scratch, int64_t recs_per_tile, double *partials,
-                 unsigned int *tickets, double *__restrict__ summary,
-                 const double *__restrict__ item_sums, int64_t chunk_begin, int64_t chunk_end,
-                 int64_t chunks_per_tile)
+/* body of k_reduce_summary.  FOCUS: the summary tiles are n planes x n_tiles grid tiles
+ * (plane-major) and plane k's per-item sums start at item_sums + k*plane_items*RT_ITEM_SUMS */
+template <bool FOCUS>
+__device__ __forceinline__ void reduce_tile(const double *__restrict__ scratch, int64_t recs_per_tile,
+                                            double *partials, unsigned int *tickets,
+                                            double *__restrict__ summary, const double *__restrict__ item_sums,
+                                            int64_t chunk_begin, int64_t chunk_end, int64_t chunks_per_tile,
+                                            int64_t n_tiles, int64_t plane_items)
 {
     __shared__ double sh[RT_RED_THREADS][RT_SUMMARY_DOUBLES + 1];
     __shared__ bool last;
     const int64_t tile = blockIdx.x/RT_RED_SPLIT;
     const int part = blockIdx.x%RT_RED_SPLIT;
+    const int64_t plane = FOCUS ? tile/n_tiles : 0;
+    const int64_t gtile = FOCUS ? tile - plane*n_tiles : tile;     /* the grid tile whose chunks it covers */
+    if (FOCUS && item_sums) item_sums += plane*plane_items*RT_ITEM_SUMS;
     const int64_t per = (recs_per_tile + RT_RED_SPLIT - 1)/RT_RED_SPLIT;
     int64_t r0 = part*per, r1 = r0 + per;
     if (r1 > recs_per_tile) r1 = recs_per_tile;
@@ -575,7 +737,7 @@ k_reduce_summary(const double *__restrict__ scratch, int64_t recs_per_tile, doub
     if (item_sums) {
         /* the work items of this tile inside the launch's chunk range, in item order: thread t of
          * part p takes items t, t + 256, ... of the part's contiguous range */
-        int64_t c0 = tile*chunks_per_tile, c1 = c0 + chunks_per_tile;
+        int64_t c0 = gtile*chunks_per_tile, c1 = c0 + chunks_per_tile;
         if (c0 < chunk_begin) c0 = chunk_begin;
         if (c1 > chunk_end) c1 = chunk_end;
         if (c1 > c0) {
@@ -621,6 +783,27 @@ k_reduce_summary(const double *__restrict__ scratch, int64_t recs_per_tile, doub
     }
 }
 
+__global__ void __launch_bounds__(RT_RED_THREADS)
+k_reduce_summary(const double *__restrict__ scratch, int64_t recs_per_tile, double *partials,
+                 unsigned int *tickets, double *__restrict__ summary,
+                 const double *__restrict__ item_sums, int64_t chunk_begin, int64_t chunk_end,
+                 int64_t chunks_per_tile)
+{
+    reduce_tile<false>(scratch, recs_per_tile, partials, tickets, summary, item_sums, chunk_begin, chunk_end,
+                       chunks_per_tile, 0, 0);
+}
+
+/* k_reduce_summary over the n planes x n_tiles summary tiles of rt_trace_grid_focus */
+__global__ void __launch_bounds__(RT_RED_THREADS)
+k_reduce_summary_focus(const double *__restrict__ scratch, int64_t recs_per_tile, double *partials,
+                       unsigned int *tickets, double *__restrict__ summary,
+                       const double *__restrict__ item_sums, int64_t chunk_begin, int64_t chunk_end,
+                       int64_t chunks_per_tile, int64_t n_tiles, int64_t plane_items)
+{
+    reduce_tile<true>(scratch, recs_per_tile, partials, tickets, summary, item_sums, chunk_begin, chunk_end,
+                      chunks_per_tile, n_tiles, plane_items);
+}
+
 /* summary of an empty chunk range: zero counts / sums, identities in the min / max columns */
 __global__ void k_summary_identity(double *__restrict__ summary, int64_t n)
 {
@@ -662,6 +845,30 @@ __global__ void k_chief_ref(const rt_surface_desc *__restrict__ g_surfs, const d
         ref_img[((int64_t)f*G.n_wvls + w)*2 + 1] = R.p.y;
     }
     if (ref_out) { ref_out[f*2 + 0] = R.p.x; ref_out[f*2 + 1] = R.p.y; }
+}
+
+/* the chief rays of k_chief_ref, their image intercepts defocused to every plane with the
+ * expression of the grid epilogue: ref_out[k][f] = p + (foc[k]/d_z) d.  blockDim.x = RT_MAX_FOCUS */
+__global__ void __launch_bounds__(RT_MAX_FOCUS)
+k_chief_ref_focus(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                  int n_ifc, GridDev G, int n_fields, int pupil_kind, int wi,
+                  const double *__restrict__ g_wvl, rt_opts o, FocusList foc, int n_foc,
+                  double *__restrict__ ref_out)
+{
+    __shared__ double s_foc[RT_MAX_FOCUS];
+    stage_focus(foc, n_foc, s_foc);
+    const int f = blockIdx.x*blockDim.x + threadIdx.x;
+    if (f >= n_fields) return;
+    Vec3 p0, d0;
+    grid_start_ray_at<false>(G, pupil_kind, f, 0.0, 0.0, false, p0, d0);
+    FullWriter fw = {nullptr, 0};
+    RayResult R;
+    trace_ray<false>(g_surfs, g_n + (int64_t)wi*n_ifc, g_wvl[wi], n_ifc, o, p0, d0, fw, R);
+    for (int k = 0; k < n_foc; k++) {
+        const double dist = div_maybe_zero(s_foc[k], R.d.z);
+        ref_out[((int64_t)k*n_fields + f)*2 + 0] = R.p.x + dist*R.d.x;
+        ref_out[((int64_t)k*n_fields + f)*2 + 1] = R.p.y + dist*R.d.y;
+    }
 }
 
 /* fp64 FMA microbenchmark: 8 independent chains per thread */
@@ -755,11 +962,12 @@ static int launch_bundle(const rt_table *t, int64_t n_rays, const double *px, co
     return RT_OK;
 }
 
-/* work counter of one launch (NULL: static schedule): a slot of the table's ring, zeroed on the stream */
-static int launch_counter(const rt_table *t, cudaStream_t stream, unsigned long long **out)
+/* work counter of one launch (NULL: static schedule, unless `always`): a slot of the table's ring,
+ * zeroed on the stream */
+static int launch_counter(const rt_table *t, cudaStream_t stream, unsigned long long **out, bool always = false)
 {
     *out = nullptr;
-    if (!t->dynamic) return RT_OK;
+    if (!t->dynamic && !always) return RT_OK;
     rt_table *tt = const_cast<rt_table *>(t);
     unsigned long long *c = t->d_counters + (tt->next_counter++ % RT_COUNTERS);
     CUDA_TRY(cudaMemsetAsync(c, 0, sizeof(unsigned long long), stream));
@@ -849,6 +1057,39 @@ static int launch_grid_lean(const rt_table *t, const GridDev &G, int64_t cb, int
 {
     return t->lean_poly ? launch_grid_lean_<OUT, SUMMARY, WAVE, true>(t, G, cb, ce, o, out, scratch, stream)
                         : launch_grid_lean_<OUT, SUMMARY, WAVE, false>(t, G, cb, ce, o, out, scratch, stream);
+}
+
+/* CTAs of the summary launch rt_trace_grid would make over [cb, ce) (per-ray outputs of kind 0):
+ * that grid decides whether the summary records are per chunk */
+static int single_focus_grid(const rt_table *t, const rt_grid *g, int64_t cb, int64_t ce, int *grid)
+{
+    int rc;
+    if (t->lean && g->pupil_kind == RT_PUPIL_EPD) {
+        const size_t smem = t->lean_bytes + RT_ACC_BYTES;
+        auto kern = t->lean_poly ? k_trace_grid_lean<0, true, false, true> : k_trace_grid_lean<0, true, false, false>;
+        if ((rc = prep_kernel(kern, smem))) return rc;
+        return persistent_grid(kern, smem, t->sm_count, ce - cb, grid);
+    }
+    const size_t smem = (t->stage ? t->stage_bytes : 0) + RT_ACC_BYTES;
+    auto kern = t->stage ? k_trace_grid<false, true, true, false> : k_trace_grid<false, true, false, false>;
+    if ((rc = prep_kernel(kern, smem))) return rc;
+    return persistent_grid(kern, smem, t->sm_count, ce - cb, grid);
+}
+
+template <typename K, typename... Args>
+static int launch_focus_kernel(K kern, size_t smem, const rt_table *t, const rt_grid *g, int64_t cb, int64_t ce,
+                               bool chunk_slots, cudaStream_t stream, Args... args)
+{
+    int rc = prep_kernel(kern, smem);
+    if (rc) return rc;
+    int grid;
+    if ((rc = persistent_grid(kern, smem, t->sm_count, ce - cb, &grid))) return rc;
+    /* per-(tile, CTA, warp) records: blockIdx.x must stay below the slots of a tile */
+    if (!chunk_slots && grid > g->chunks_per_tile) grid = (int)g->chunks_per_tile;
+    kern<<<grid, RT_BLOCK, smem, stream>>>(args...);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
 }
 
 /* 0: p,d only; 1: + normal/dst; 2: whole ray */
@@ -1304,6 +1545,117 @@ int rt_grid_chief_ref(const rt_table *t, rt_grid *g, int32_t wvl_idx, double *re
     k_chief_ref<<<blocks, threads, 0, (cudaStream_t)stream>>>(t->d_surfs, t->d_n, t->n_ifc, grid_dev(g),
                                                               g->n_fields, g->pupil_kind, wvl_idx, t->d_wvl,
                                                               o, g->d_ref_img, ref_out);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+static int check_focus(const char *fn, const double *foc, int32_t n_foc, FocusList *L)
+{
+    if (n_foc < 1 || n_foc > RT_MAX_FOCUS) return fail(RT_ERR_INVALID, "%s: n_foc must be in [1, RT_MAX_FOCUS]", fn);
+    if (!foc) return fail(RT_ERR_INVALID, "%s: foc is NULL", fn);
+    memset(L, 0, sizeof *L);
+    for (int k = 0; k < n_foc; k++) {
+        if (!std::isfinite(foc[k])) return fail(RT_ERR_INVALID, "%s: foc holds a value that is not finite", fn);
+        L->v[k] = foc[k];
+    }
+    return RT_OK;
+}
+
+int rt_grid_chief_ref_focus(const rt_table *t, const rt_grid *g, int32_t wvl_idx, const double *foc,
+                            int32_t n_foc, double *ref_out, void *stream)
+{
+    FocusList L;
+    int rc = check_focus("rt_grid_chief_ref_focus", foc, n_foc, &L);
+    if (rc) return rc;
+    if (!t || !g || !ref_out) return fail(RT_ERR_INVALID, "rt_grid_chief_ref_focus: bad arguments");
+    if (t->device != g->device) return fail(RT_ERR_INVALID, "rt_grid_chief_ref_focus: table and grid on different devices");
+    if (wvl_idx < 0 || wvl_idx >= t->n_wvl) return fail(RT_ERR_INVALID, "rt_grid_chief_ref_focus: wvl_idx out of range");
+    DeviceGuard guard(t->device);
+    rt_opts o;     /* as rt_grid_chief_ref */
+    o.eps = 1.0e-12; o.pt_inside_fuzz = -1.0; o.check_apertures = 0; o.intersect_obj = 1;
+    o.filter_out_phantoms = 0; o.first_surf = 1; o.last_surf = t->n_ifc - 2; o.wvl_idx = wvl_idx;
+    const int threads = RT_MAX_FOCUS, blocks = (g->n_fields + threads - 1)/threads;
+    k_chief_ref_focus<<<blocks, threads, 0, (cudaStream_t)stream>>>(t->d_surfs, t->d_n, t->n_ifc, grid_dev(g),
+                                                                    g->n_fields, g->pupil_kind, wvl_idx, t->d_wvl,
+                                                                    o, L, n_foc, ref_out);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+int64_t rt_grid_focus_scratch_bytes(const rt_grid *g, int32_t n_foc, int64_t chunk_begin, int64_t chunk_end)
+{
+    if (!g || n_foc < 1 || n_foc > RT_MAX_FOCUS || chunk_end < chunk_begin) return 0;
+    return n_foc*rt_grid_scratch_bytes(g, chunk_begin, chunk_end);
+}
+
+/* scratch: records [n][n_tiles][slots][RT_WARPS][16] | partials [n*n_tiles][RT_RED_SPLIT][16] |
+ * tickets [n*n_tiles] | per-item sums [n][items][RT_ITEM_SUMS] */
+int rt_trace_grid_focus(const rt_table *t, const rt_grid *g, int64_t chunk_begin, int64_t chunk_end,
+                        const rt_opts *o, const double *foc, int32_t n_foc, const double *ref_img,
+                        const rt_out *out, double *summary, void *scratch, void *stream)
+{
+    FocusList L;
+    int rc = check_focus("rt_trace_grid_focus", foc, n_foc, &L);
+    if (rc) return rc;
+    if (!summary) return fail(RT_ERR_INVALID, "rt_trace_grid_focus: summary is NULL");
+    if (!out) return fail(RT_ERR_INVALID, "rt_trace_grid_focus: out is NULL");
+    if (out->abr_x || out->abr_y || out->opd || out->full)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_focus: abr_x, abr_y, opd and full must be NULL (they depend on the plane)");
+    if (out_kind(out) != 0)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_focus: normals and dst are not written by the through-focus trace");
+    if (!t || !g || !scratch) return fail(RT_ERR_INVALID, "rt_trace_grid_focus: bad arguments");
+    if (t->device != g->device) return fail(RT_ERR_INVALID, "rt_trace_grid_focus: table and grid on different devices");
+    if (chunk_begin < 0 || chunk_end > g->n_chunks || chunk_end < chunk_begin)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_focus: chunk range out of bounds");
+    if ((rc = check_opts(t, o))) return rc;
+    for (int32_t wi : g->h_wvl_idx)
+        if (wi < 0 || wi >= t->n_wvl)
+            return fail(RT_ERR_INVALID, "rt_trace_grid_focus: the grid's wvl_idx is out of range for this table");
+    DeviceGuard guard(t->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const int64_t n_sum = (int64_t)n_foc*g->n_tiles;      /* summary tiles, plane-major */
+    if (chunk_begin == chunk_end) {
+        const int64_t n = n_sum*RT_SUMMARY_DOUBLES;
+        k_summary_identity<<<(unsigned)((n + 255)/256), 256, 0, s>>>(summary, n);
+        g_launches++;
+        CUDA_TRY(cudaGetLastError());
+        return RT_OK;
+    }
+    int single;
+    if ((rc = single_focus_grid(t, g, chunk_begin, chunk_end, &single))) return rc;
+    const bool chunk_slots = g->chunks_per_tile <= single;
+    double *scr = (double *)scratch;
+    const int64_t recs = scratch_records(g);                 /* per plane */
+    double *partials = scr + n_foc*recs*RT_SUMMARY_DOUBLES;
+    unsigned int *tickets = (unsigned int *)(partials + n_sum*RT_RED_SPLIT*RT_SUMMARY_DOUBLES);
+    double *items = scr + n_foc*scratch_head_doubles(g);
+    /* the per-item sums are all written by the trace: zero the records, partials and tickets only */
+    CUDA_TRY(cudaMemsetAsync(scr, 0, (size_t)(n_foc*scratch_head_doubles(g))*sizeof(double), s));
+    unsigned long long *wc;
+    if ((rc = launch_counter(t, s, &wc, true))) return rc;
+    FocusPlanes P;
+    P.foc = nullptr; P.ref = ref_img; P.n_tiles = g->n_tiles;
+    P.n_items = (chunk_end - chunk_begin)*RT_WARPS;
+    P.n = n_foc; P.n_fields = g->n_fields; P.chunk_slots = chunk_slots; P.pad_ = 0;
+    const GridDev G = grid_dev(g);
+    /* angular pupil specifications are generated by the general kernels only (rt_grid.cuh) */
+    if (t->lean && g->pupil_kind == RT_PUPIL_EPD) {
+        auto kern = t->lean_poly ? k_trace_grid_lean_focus<true> : k_trace_grid_lean_focus<false>;
+        rc = launch_focus_kernel(kern, t->lean_bytes, t, g, chunk_begin, chunk_end, chunk_slots, s,
+                                 t->d_surfs, t->d_n, t->n_ifc, t->n_wvl, G, chunk_begin, chunk_end, *o, *out,
+                                 scr, wc, items, P, L);
+    } else {
+        auto kern = t->stage ? k_trace_grid_focus<true> : k_trace_grid_focus<false>;
+        rc = launch_focus_kernel(kern, t->stage ? t->stage_bytes : 0, t, g, chunk_begin, chunk_end, chunk_slots, s,
+                                 t->d_surfs, t->d_n, t->n_ifc, t->n_wvl, G, chunk_begin, chunk_end, *o, *out,
+                                 scr, t->d_wvl, g->pupil_kind, wc, items, P, L);
+    }
+    if (rc) return rc;
+    k_reduce_summary_focus<<<(unsigned)(n_sum*RT_RED_SPLIT), RT_RED_THREADS, 0, s>>>(
+        scr, recs/g->n_tiles, partials, tickets, summary, chunk_slots ? nullptr : items, chunk_begin, chunk_end,
+        g->chunks_per_tile, g->n_tiles, P.n_items);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RT_OK;

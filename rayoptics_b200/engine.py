@@ -327,6 +327,20 @@ class PupilGrid(PupilGridSpec):
                                                    _stream_ptr(torch.device('cuda', self.device))))
         return out
 
+    def chief_ref_focus(self, table, wvl_idx, foc, out=None):
+        """The chief rays of ``chief_ref``, their image intercepts defocused to every focus shift
+        of ``foc`` (``rt_grid_chief_ref_focus``): ``[K, n_fields, 2]`` float64 device tensor
+        (``out`` if given).  The grid's own reference points are not changed."""
+        foc = _focus_array(foc)
+        if out is None:
+            out = torch.empty((len(foc), self.n_fields, 2), dtype=torch.float64,
+                              device=torch.device('cuda', self.device))
+        with torch.cuda.device(self.device):
+            _abi.check(self._lib.rt_grid_chief_ref_focus(
+                table.handle, self.handle, int(wvl_idx), foc.ctypes.data_as(_abi.c_double_p), len(foc),
+                _ptr(out), _stream_ptr(torch.device('cuda', self.device))))
+        return out
+
     def close(self):
         if getattr(self, '_handle', None) is not None:
             self._lib.rt_grid_destroy(self._handle)
@@ -377,6 +391,48 @@ def trace_grid(table, grid, chunk_begin=0, chunk_end=None, outputs=GRID_OUTPUTS,
     res.summary = summ
     res._keep = scratch
     return res
+
+
+def _focus_array(foc):
+    return np.ascontiguousarray(np.atleast_1d(np.asarray(foc, dtype=np.float64)).ravel())
+
+
+def trace_grid_focus(table, grid, foc, chunk_begin=0, chunk_end=None, ref_img=None, res=None, **kwargs):
+    """Spot sums of chunks ``[chunk_begin, chunk_end)`` of a PupilGrid at every focus shift of
+    ``foc`` from one trace (``rt_trace_grid_focus``): ``[K, n_tiles, 16]`` float64 device tensor
+    whose row k is the ``trace_grid`` summary of the grid with ``foc = foc[k]``.  ``ref_img``:
+    ``[K, n_fields, 2]`` device tensor of reference image points per plane (``chief_ref_focus``)
+    or None (= 0).  ``res``: optional BundleResult that receives the per-ray ``p``, ``d``,
+    ``op``, ``status``, ``fail_surf``, ``n_seg`` (the aberrations depend on the plane and are not
+    written).  Trace defaults as ``trace_grid``.  Asynchronous on the current CUDA stream."""
+    lib = _abi.load_library()
+    device = torch.device('cuda', table.device)
+    foc = _focus_array(foc)
+    if chunk_end is None:
+        chunk_end = grid.n_chunks
+    kwargs.setdefault('check_apertures', True)
+    kwargs.setdefault('first_surf', 1)
+    kwargs.setdefault('last_surf', table.n_ifc - 2)
+    if grid.pupil_kind == _abi.PUPIL_WIDE:
+        kwargs['intersect_obj'] = False
+    opts = _abi.make_opts(**kwargs)
+    if res is None:
+        res = BundleResult(0, table.n_ifc, device, ())
+    elif res.n != grid.rays_in_chunks(chunk_begin, chunk_end):
+        raise ValueError('res was allocated for a different number of rays')
+    out = res.c_struct()
+    if ref_img is not None:
+        if tuple(ref_img.shape) != (len(foc), grid.n_fields, 2) or ref_img.dtype != torch.float64 \
+                or ref_img.device != device or not ref_img.is_contiguous():
+            raise ValueError('ref_img must be a contiguous float64 [K, n_fields, 2] tensor on the table\'s device')
+    summ = torch.empty((len(foc), grid.n_tiles, RT_SUMMARY_DOUBLES), dtype=torch.float64, device=device)
+    nbytes = lib.rt_grid_focus_scratch_bytes(grid.handle, len(foc), chunk_begin, chunk_end)
+    scratch = torch.empty(max(nbytes//8, 1), dtype=torch.float64, device=device)
+    _abi.check(lib.rt_trace_grid_focus(table.handle, grid.handle, chunk_begin, chunk_end, C.byref(opts),
+                                       foc.ctypes.data_as(_abi.c_double_p), len(foc), _ptr(ref_img),
+                                       C.byref(out), _ptr(summ), _ptr(scratch), _stream_ptr(device)))
+    summ._keep = (scratch, ref_img)      # inputs / scratch must outlive the asynchronous launches
+    return summ
 
 
 def trace_grid_to_host(table, grid, h_abr, chunk_begin=0, chunk_end=None, pieces=8, summary=True,
