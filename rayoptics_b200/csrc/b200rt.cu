@@ -142,12 +142,15 @@ __device__ __forceinline__ void stage_table(const rt_surface_desc *g_surfs, cons
     }
 }
 
+/* NRML == false: a launch of output kind 0 (out_kind), whose normal and dst columns are NULL,
+ * so that R.n and R.dst need not be formed */
+template <bool NRML>
 __device__ __forceinline__ void store_result(const rt_out &out, int64_t k, const RayResult &R)
 {
     if (out.px) { out.px[k] = R.p.x; out.py[k] = R.p.y; out.pz[k] = R.p.z; }
     if (out.dx) { out.dx[k] = R.d.x; out.dy[k] = R.d.y; out.dz[k] = R.d.z; }
-    if (out.nx) { out.nx[k] = R.n.x; out.ny[k] = R.n.y; out.nz[k] = R.n.z; }
-    if (out.dst) out.dst[k] = R.dst;
+    if (NRML && out.nx) { out.nx[k] = R.n.x; out.ny[k] = R.n.y; out.nz[k] = R.n.z; }
+    if (NRML && out.dst) out.dst[k] = R.dst;
     if (out.op) out.op[k] = R.op;
     if (out.status) out.status[k] = R.status;
     if (out.fail_surf) out.fail_surf[k] = R.fail_surf;
@@ -177,7 +180,7 @@ k_trace_bundle(const rt_surface_desc *__restrict__ g_surfs, const double *__rest
         FullWriter fw = {FULL ? out.full + r : nullptr, out.full_stride};
         RayResult R;
         trace_ray<FULL>(tab, ntab + (int64_t)w*n_ifc, g_wvl[w], n_ifc, o, p0, d0, fw, R);
-        store_result(out, r, R);
+        store_result<true>(out, r, R);
     }
 }
 
@@ -408,8 +411,8 @@ __device__ __forceinline__ void focus_item(const FocusPlanes &F, bool have, int 
 /* chunk loop shared by the general and the lean grid kernels: start ray ->
  * trace -> per-ray results -> transverse aberration (focus_pupil_coords,
  * analyses.py:561-580) -> spot sums.  FOCUS: the spot sums of the planes of *FP instead
- * (needs SUMMARY == false and a work counter). */
-template <bool SUMMARY, bool WAVE, bool FOCUS = false, typename TraceFn>
+ * (needs SUMMARY == false and a work counter).  NRML: see store_result. */
+template <bool SUMMARY, bool WAVE, bool FOCUS = false, bool NRML = true, typename TraceFn>
 __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_begin, int64_t chunk_end,
                                                 const rt_out &out, double *scratch, double *acc,
                                                 unsigned long long *work_counter, double *item_sums,
@@ -461,7 +464,7 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             RayResult R;
             Vec3 d0;
             trace(f, w, loc, k, R, d0);
-            store_result(out, k, R);
+            store_result<NRML>(out, k, R);
             status = R.status; op = R.op;
             if (FOCUS) { fp = R.p; fd = R.d; }
             if (WAVE)
@@ -580,7 +583,7 @@ k_trace_bundle_lean(const rt_surface_desc *__restrict__ g_surfs, const double *_
         FullWriter fw = {OUT == 2 ? out.full + r : nullptr, out.full_stride};
         RayResult R;
         trace_ray_lean<OUT, false, POLY>(ls, li + (int64_t)w*n_ifc, lp, g_surfs, n_ifc, o, p0, d0, fw, R);
-        store_result(out, r, R);
+        store_result<(OUT >= 1)>(out, r, R);
     }
 }
 
@@ -599,7 +602,7 @@ k_trace_grid_lean(const rt_surface_desc *__restrict__ g_surfs, const double *__r
     build_plan(g_surfs, g_n, n_ifc, n_wvl, o, ls, li);
     if (POLY) build_poly_plan(g_surfs, n_ifc, lp);
     __syncthreads();
-    grid_chunk_loop<SUMMARY, WAVE>(G, chunk_begin, chunk_end, out, scratch, acc, work_counter, item_sums,
+    grid_chunk_loop<SUMMARY, WAVE, false, (OUT >= 1)>(G, chunk_begin, chunk_end, out, scratch, acc, work_counter, item_sums,
         [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0) {
             Vec3 p0;
             grid_start_ray<true>(G, RT_PUPIL_EPD, f, loc, p0, d0);
@@ -626,7 +629,7 @@ k_trace_grid_lean_focus(const rt_surface_desc *__restrict__ g_surfs, const doubl
     stage_focus(foc, P.n, s_foc);                /* its barrier also completes the plan */
     FocusPlanes F = P;
     F.foc = s_foc;
-    grid_chunk_loop<false, false, true>(G, chunk_begin, chunk_end, out, scratch, nullptr, work_counter, item_sums,
+    grid_chunk_loop<false, false, true, false>(G, chunk_begin, chunk_end, out, scratch, nullptr, work_counter, item_sums,
         [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0) {
             Vec3 p0;
             grid_start_ray<true>(G, RT_PUPIL_EPD, f, loc, p0, d0);
