@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define RT_ABI_VERSION 5
+#define RT_ABI_VERSION 6
 #define RT_MAX_COEFS 20     /* EvenPolynomial uses <=10, RadialPolynomial <=20 */
 #define RT_MAX_PHASE_COEFS 10
 #define RT_MAX_APERTURES 4  /* Surface.clear_apertures entries honoured per interface */
@@ -43,6 +43,7 @@ extern "C" {
 #define RT_SUMMARY_DOUBLES 16
 #define RT_WAVE_DOUBLES 24   /* per-(field, wvl) chief-ray / reference-sphere record, see rt_grid_spec.wave */
 #define RT_MAX_FOCUS 64      /* image planes of one rt_trace_grid_focus call */
+#define RT_WFE_DOUBLES 24    /* per-tile wavefront-error record of rt_trace_grid_wfe */
 
 /* error codes (function return values) */
 enum rt_error {
@@ -362,6 +363,33 @@ int rt_trace_grid_focus(const rt_table *table, const rt_grid *grid,
  * min / max.  One launch on `stream`. */
 int rt_combine_summaries(const double *parts, int32_t n_parts, int64_t n_tiles,
                          double *out, void *stream);
+
+/* ---- wavefront error (ABI 6): the sums behind RMS / P-V wavefront error and its least-squares
+ * fits on {1, x, y} and {1, x, y, r^2}, per tile, from one grid trace with the OPD epilogue.
+ * W = the ray's opd (system units) as rt_trace_grid writes it; (x, y) = the ray's relative pupil
+ * coordinates pupil_x[i], pupil_y[j] of its rt_grid_spec, after Field.apply_vignetting when the grid
+ * applies it; r2 = x*x + y*y.  summary: DEVICE [n_tiles][RT_WFE_DOUBLES]:
+ *   0 n_ok 1 n_missed 2 n_tir 3 n_blocked 4 n_other   (as the spot summary)
+ *   5 min W 6 max W                                    (fmin / fmax: NaN skipped; +-inf without rays)
+ *   7 sum W 8 sum W*W 9 sum x*W 10 sum y*W 11 sum r2*W
+ *   12 sum x 13 sum y 14 sum x*x 15 sum x*y 16 sum y*y 17 sum x*r2 18 sum y*r2 19 sum r2*r2
+ *   20-23 reserved (0)
+ * Only status-0 rays enter columns 5-19; a status-0 ray with a NaN opd makes its tile's sums NaN.
+ * The sums are added in the fixed order of DESIGN.md section 4 (32-ray work items drawn from a
+ * counter, each summed by one shuffle tree and stored on its own): bit-reproducible.  B200RT_STATIC
+ * does not apply. */
+/* DEVICE scratch bytes of rt_trace_grid_wfe over [chunk_begin, chunk_end); 0 for bad arguments */
+int64_t rt_grid_wfe_scratch_bytes(const rt_grid *grid, int64_t chunk_begin, int64_t chunk_end);
+/* The grid must carry rt_grid_spec.wave.  out: per-ray results as rt_trace_grid (opd included,
+ * all optional); out.full must be NULL.  summary and scratch are required.  RT_ERR_INVALID before
+ * any device work for bad arguments.  Two kernel launches (one for an empty chunk range). */
+int rt_trace_grid_wfe(const rt_table *table, const rt_grid *grid,
+                      int64_t chunk_begin, int64_t chunk_end, const rt_opts *opts,
+                      const rt_out *out, double *summary, void *scratch, void *stream);
+/* rt_combine_summaries for wavefront-error records: parts DEVICE [n_parts][n_tiles][RT_WFE_DOUBLES]
+ * -> out DEVICE [n_tiles][RT_WFE_DOUBLES]; sums and counts add in part order, column 5 takes fmin,
+ * column 6 fmax.  One launch on `stream`. */
+int rt_combine_wfe(const double *parts, int32_t n_parts, int64_t n_tiles, double *out, void *stream);
 
 /* ---- misc */
 const char *rt_last_error(void);

@@ -315,6 +315,113 @@ def through_focus(opt_model, num_rays=21, foc=None, num_planes=21, fields=None, 
     return ThroughFocus(foc, stats, ref, num_rays, nf, nw)
 
 
+class WavefrontError:
+    """Result of ``wavefront_error``: ``[n_fields, n_wvls]`` arrays, in waves, of
+
+    ``rms`` (piston removed), ``pv``, ``rms_tilt`` / ``tilt_x`` / ``tilt_y`` (least-squares fit on
+    {1, x, y}), ``rms_focus`` / ``focus`` (fit on {1, x, y, r^2}; coefficients at unit relative
+    pupil), and the ray counts ``n_ok``, ``n_missed``, ``n_tir``, ``n_blocked``, ``n_other``
+    (``engine.wavefront_statistics``).  ``summary``: the combined ``[n_tiles, RT_WFE_DOUBLES]``
+    sums; ``ref_img`` ``[n_fields, n_wvls, 2]``: the reference image points; ``num_rays``: pupil
+    samples per side."""
+
+    def __init__(self, stats, summary, ref_img, num_rays, n_fields, n_wvls):
+        self.stats = {k: np.asarray(v).reshape(n_fields, n_wvls) for k, v in stats.items()}
+        for k, v in self.stats.items():
+            setattr(self, k, v)
+        self.summary, self.ref_img = summary, ref_img
+        self.num_rays, self.n_fields, self.n_wvls = num_rays, n_fields, n_wvls
+
+
+def _wavefront_pupil(opt_model, fld, num_rays):
+    """pupil samples of ``RayGrid``: ``num_rays`` accumulated steps over the field's vignetting
+    bounding box (Field.vignetting_bbox, oversize 1)"""
+    poly = np.array([fld.apply_vignetting(list(pr)) for pr in opt_model.optical_spec.pupil.pupil_rays])
+    lo, hi = poly.min(axis=0), poly.max(axis=0)
+    return (E.accumulated_steps(lo[0], hi[0], num_rays), E.accumulated_steps(lo[1], hi[1], num_rays))
+
+
+def _wfe_sums_host(spec, status, opd):
+    """The ``[n_tiles, RT_WFE_DOUBLES]`` record of traced rays, formed on the host (the
+    ``backend=`` test seam; the device forms it in ``rt_trace_grid_wfe``)."""
+    from ._abi import RT_WFE_DOUBLES
+    s = np.zeros((spec.n_tiles, RT_WFE_DOUBLES))
+    per = spec.rays_per_tile
+    for t in range(spec.n_tiles):
+        f = t//spec.n_wvls
+        gx, gy = np.meshgrid(spec.pupil_x[f], spec.pupil_y[f], indexing='ij')
+        st, w = status[t*per:(t + 1)*per], opd[t*per:(t + 1)*per]
+        ok = st == 0
+        cls = np.where((st >= 0) & (st <= 3), st, 4)
+        s[t, 0:5] = np.bincount(cls, minlength=5)[:5]
+        x, y, w = gx.ravel()[ok], gy.ravel()[ok], w[ok]
+        r2 = x*x + y*y
+        s[t, 5] = np.fmin.reduce(w, initial=np.inf)
+        s[t, 6] = np.fmax.reduce(w, initial=-np.inf)
+        s[t, 7:20] = [v.sum() for v in (w, w*w, x*w, y*w, r2*w, x, y, x*x, x*y, y*y, x*r2, y*r2, r2*r2)]
+    return s
+
+
+def wavefront_grid_args(opt_model, table, num_rays, fields, wvls, foc, image_pt_2d=None, image_delta=None,
+                        backend=None):
+    """``(args, kw)`` of the PupilGridSpec / PupilGrid that ``wavefront_error`` traces: the chief rays
+    and reference spheres of all tiles (one ``waveabr.setup_tiles`` call), each field's ``RayGrid``
+    pupil samples, no vignetting applied"""
+    sm = opt_model.seq_model
+    wave, ref_img, _ = W.setup_tiles(opt_model, table, fields, wvls, foc, image_pt_2d, image_delta,
+                                     chief_tracer=None if backend is None else backend.chief_rays)
+    pupils = [_wavefront_pupil(opt_model, fld, num_rays) for fld in fields]
+    recs, eprad, z_pupil = grid_fields_of(opt_model, fields)
+    wvl_idx = [sm.index_for_wavelength(w) if table is None else table.wvl_index(w) for w in wvls]
+    args = (recs, wvl_idx, np.array([p[0] for p in pupils]), np.array([p[1] for p in pupils]), eprad, z_pupil)
+    return args, dict(ref_img=ref_img, apply_vignetting=False, flip_z_dir=sm.z_dir[0], foc=foc, wave=wave)
+
+
+def wavefront_error(opt_model, num_rays=21, fields=None, wvls=None, foc=None, image_pt_2d=None,
+                    image_delta=None, table=None, device=0, shard=None, group=None, chunk_range=None,
+                    backend=None, **kwargs):
+    """RMS and P-V wavefront error, with tilt and with tilt + focus removed, of every field and
+    wavelength from one grid trace.
+
+    Tile (field f, wavelength w) holds the rays of ``RayGrid(opt_model, f, w, foc,
+    num_rays=num_rays)``: the same square grid over the field's vignetting bounding box, no
+    vignetting applied, apertures checked, the same chief ray and reference sphere.  The chief rays
+    and reference spheres of all tiles come from one ``waveabr.setup_tiles`` call, the OPDs are
+    reduced on the device to per-tile sums (``rt_trace_grid_wfe``) and only those sums come back.
+    ``shard=(rank, world)`` / ``group`` / ``chunk_range`` as ``spot_diagram``: one all-gather of
+    the ``[n_tiles, RT_WFE_DOUBLES]`` sums.  ``backend``: the CPU test seam of ``RayGrid``.
+    ``kwargs``: trace options (``check_apertures``, ...).  Returns a ``WavefrontError``."""
+    from .parallel import shard_chunks, gather_summaries
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    fields = list(osp.field_of_view.fields if fields is None else fields)
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    foc = osp.defocus.focus_shift if foc is None else foc
+    tab = None if backend is not None else _table_for(opt_model, table, device)
+    args, grid_kw = wavefront_grid_args(opt_model, tab, num_rays, fields, wvls, foc, image_pt_2d, image_delta,
+                                        backend)
+    ref_img = grid_kw['ref_img']
+    kwargs.setdefault('check_apertures', True)
+    if backend is not None:
+        spec = E.PupilGridSpec(*args, **grid_kw)
+        r = backend.trace_tile(opt_model, spec, True, kwargs['check_apertures'])
+        summ_host = _wfe_sums_host(spec, np.asarray(r['status']), np.asarray(r['opd']))
+    else:
+        dev = torch.device('cuda', tab.device)
+        with torch.cuda.device(dev):
+            grid = E.PupilGrid(*args, device=tab.device, **grid_kw)
+            c0, c1 = (0, grid.n_chunks) if shard is None else shard_chunks(grid.n_chunks, *shard)
+            if chunk_range is not None:
+                c0, c1 = chunk_range
+            summ = E.trace_grid_wfe(tab, grid, c0, c1, **kwargs)
+            if shard is not None:
+                summ = gather_summaries(summ, group)
+            summ_host = summ.cpu().numpy()                 # one small copy; waits
+            grid.close()
+    lam = np.array([[opt_model.nm_to_sys_units(w) for w in wvls]]*len(fields)).ravel()
+    stats = E.wavefront_statistics(summ_host, lam)
+    return WavefrontError(stats, summ_host, ref_img, num_rays, len(fields), len(wvls))
+
+
 # --------------------------------------------------------------------------
 # RayFan / RayList / RayGrid: the reference's analysis classes
 # (/root/reference/src/rayoptics/raytr/analyses.py:121-187,343-434,584-663) with

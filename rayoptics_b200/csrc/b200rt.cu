@@ -8,7 +8,9 @@
  *                               (field, wavelength, pupil i, j) index, optional
  *                               per-chunk spot sums
  *   k_trace_grid[_lean]_focus   one trace, spot sums at up to RT_MAX_FOCUS image planes
- *   k_reduce_summary            fixed-order per-tile reduction of the chunk sums
+ *   k_trace_grid[_lean]_wfe     one trace, per-tile sums of the OPD and its least-squares fits
+ *   k_reduce_summary            fixed-order per-tile reduction of the chunk sums (_wfe: of the
+ *                               wavefront-error sums)
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
  * The surface table (n_ifc x rt_surface_desc + n_wvl x n_ifc indices) is staged
@@ -408,16 +410,101 @@ __device__ __forceinline__ void focus_item(const FocusPlanes &F, bool have, int 
     }
 }
 
+/* ---- wavefront-error sums (rt_trace_grid_wfe): per work item, the 13 sums of W = opd and the
+ * relative pupil coordinates (x, y) of its status-0 rays (RT_WFE_DOUBLES columns 7-19), and per
+ * (tile, CTA, warp) a record of the counts and min / max W, whose result does not depend on the
+ * order the rays are added in.  Always drawn from a work counter. */
+#define RT_WFE_ITEM_SUMS 13
+
+/* the 13 sums of one work item in 8 + 4 + 2 + 1 + 1 = 16 shuffles: the transposition of
+ * item_sums_store widened to 16 slots.  At the 16 / 8 / 4 / 2 exchanges every lane hands over the
+ * half of its values that its partner keeps; the additions are the halving tree x[i] + x[i+16],
+ * +8, +4, +2, +1 of every value (DESIGN.md section 4).  Summands, formed unfused in this order:
+ * W, W*W, x*W, y*W, r2*W, x, y, x*x, x*y, y*y, x*r2, y*r2, r2*r2 with r2 = x*x + y*y; lanes
+ * without a status-0 ray hold +0.0. */
+__device__ __forceinline__ void wfe_item_sums_store(bool ok, double W, double x, double y, double *dst)
+{
+    const int lane = threadIdx.x & 31;
+    const double r2 = x*x + y*y;
+    double v[16];
+    v[0] = W; v[1] = W*W; v[2] = x*W; v[3] = y*W; v[4] = r2*W;
+    v[5] = x; v[6] = y; v[7] = x*x; v[8] = x*y; v[9] = y*y;
+    v[10] = x*r2; v[11] = y*r2; v[12] = r2*r2; v[13] = 0.0; v[14] = 0.0; v[15] = 0.0;
+#pragma unroll
+    for (int k = 0; k < RT_WFE_ITEM_SUMS; k++) v[k] = ok ? v[k] : 0.0;
+    const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4, h2 = lane & 2;
+    /* 16: lower half-warp keeps v0..v7, upper keeps v8..v15 */
+    double a[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++)
+        a[k] = (h16 ? v[8 + k] : v[k]) + __shfl_xor_sync(0xffffffffu, h16 ? v[k] : v[8 + k], 16);
+    /* 8: keep a0..a3 | a4..a7 */
+    double b[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        b[k] = (h8 ? a[4 + k] : a[k]) + __shfl_xor_sync(0xffffffffu, h8 ? a[k] : a[4 + k], 8);
+    /* 4: keep b0, b1 | b2, b3 */
+    const double c0 = (h4 ? b[2] : b[0]) + __shfl_xor_sync(0xffffffffu, h4 ? b[0] : b[2], 4);
+    const double c1 = (h4 ? b[3] : b[1]) + __shfl_xor_sync(0xffffffffu, h4 ? b[1] : b[3], 4);
+    /* 2: keep c0 | c1 */
+    double e = (h2 ? c1 : c0) + __shfl_xor_sync(0xffffffffu, h2 ? c0 : c1, 2);
+    e = e + __shfl_xor_sync(0xffffffffu, e, 1);
+    /* lane 2g holds value index 8*[bit 4] + 4*[bit 3] + 2*[bit 2] + [bit 1] of g = lane/2 */
+    const int idx = ((lane >> 4) & 1)*8 + ((lane >> 3) & 1)*4 + ((lane >> 2) & 1)*2 + ((lane >> 1) & 1);
+    if ((lane & 1) == 0 && idx < RT_WFE_ITEM_SUMS) dst[idx] = e;
+}
+
+/* one work item of the wavefront-error trace: its sums, and its counts / min / max folded into the
+ * warp's record of the tile (overwritten when the warp meets the tile first) */
+__device__ __forceinline__ void wfe_item(bool have, int status, double W, double x, double y, int64_t tile,
+                                         bool first, int64_t sl, double *scratch, double *item_dst)
+{
+    const int lane = threadIdx.x & 31;
+    const bool ok = have && status == RT_RAY_OK;
+    wfe_item_sums_store(ok, W, x, y, item_dst);
+    const int ck = status == RT_RAY_OK ? 0 : (status <= RT_RAY_BLOCKED ? status : 4);
+    double cnt = 0.0;
+#pragma unroll
+    for (int c = 0; c < 5; c++) {
+        const unsigned m = __ballot_sync(0xffffffffu, have && ck == c);
+        if (lane == c + 1) cnt = (double)__popc(m);
+    }
+    /* min / max in 5 shuffles: the lower half-warp reduces min, the upper max; lanes 0 and 16 */
+    const bool h16 = lane & 16;
+    const double mn = ok ? W : CUDART_INF, mx = ok ? W : -CUDART_INF;
+    const double got = __shfl_xor_sync(0xffffffffu, h16 ? mn : mx, 16);
+    double b = h16 ? fmax(mx, got) : fmin(mn, got);
+#pragma unroll
+    for (int s = 8; s > 0; s >>= 1) {
+        const double o = __shfl_xor_sync(0xffffffffu, b, s);
+        b = h16 ? fmax(b, o) : fmin(b, o);
+    }
+    /* record column this lane writes: 5 min (lane 0), 6 max (lane 16), 0..4 the counts (lanes 1..5),
+     * 20 the valid flag (lane 6) */
+    const int col = lane == 0 ? 5 : lane == 16 ? 6 : (lane >= 1 && lane <= 5) ? lane - 1 : (lane == 6 ? 20 : -1);
+    if (col < 0) return;
+    double *dst = scratch + ((tile*sl + blockIdx.x)*RT_WARPS + (threadIdx.x >> 5))*RT_WFE_DOUBLES;
+    double v = col == 5 || col == 6 ? b : (col == 20 ? 1.0 : cnt);
+    /* a warp's items come in increasing order, so it never returns to a tile it has left */
+    if (!first && col != 20) {
+        const double o = dst[col];
+        v = col == 5 ? fmin(o, v) : col == 6 ? fmax(o, v) : o + v;
+    }
+    dst[col] = v;
+}
+
 /* chunk loop shared by the general and the lean grid kernels: start ray ->
  * trace -> per-ray results -> transverse aberration (focus_pupil_coords,
  * analyses.py:561-580) -> spot sums.  FOCUS: the spot sums of the planes of *FP instead
- * (needs SUMMARY == false and a work counter).  NRML: see store_result. */
-template <bool SUMMARY, bool WAVE, bool FOCUS = false, bool NRML = true, typename TraceFn>
+ * (needs SUMMARY == false and a work counter).  WFE: the wavefront-error sums of wfe_item instead
+ * (needs WAVE, SUMMARY == false and a work counter).  NRML: see store_result. */
+template <bool SUMMARY, bool WAVE, bool FOCUS = false, bool NRML = true, bool WFE = false, typename TraceFn>
 __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_begin, int64_t chunk_end,
                                                 const rt_out &out, double *scratch, double *acc,
                                                 unsigned long long *work_counter, double *item_sums,
                                                 TraceFn trace, const FocusPlanes *FP = nullptr)
 {
+    static_assert(!WFE || (WAVE && !SUMMARY && !FOCUS), "WFE needs the OPD epilogue and no spot sums");
     const int64_t tile0 = chunk_begin/G.chunks_per_tile;
     const int64_t ray0 = tile0*G.rays_per_tile + (chunk_begin - tile0*G.chunks_per_tile)*RT_BLOCK;
     const int64_t sl = G.chunks_per_tile < RT_MAX_GRID ? G.chunks_per_tile : RT_MAX_GRID;
@@ -457,6 +544,7 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
         int status = RT_RAY_OK;
         double ax = 0.0, ay = 0.0, op = 0.0;
         Vec3 fp = {0.0, 0.0, 0.0}, fd = {0.0, 0.0, 0.0};     /* FOCUS: image point and direction */
+        double wW = 0.0, wx = 0.0, wy = 0.0;                  /* WFE: opd, relative pupil coordinates */
         if (have) {
             const int f = (int)(tile/G.n_wvls);
             const int w = (int)(tile - (int64_t)f*G.n_wvls);
@@ -467,10 +555,16 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             store_result<NRML>(out, k, R);
             status = R.status; op = R.op;
             if (FOCUS) { fp = R.p; fd = R.d; }
-            if (WAVE)
-                out.opd[k] = (R.status == RT_RAY_OK)
-                                 ? wave_opd(G.wave + tile*RT_WAVE_DOUBLES, R.p1, d0, R.pk, R.dk, R.p, R.d, R.op)
-                                 : CUDART_NAN;
+            if (WAVE) {
+                const double opd = (R.status == RT_RAY_OK)
+                                       ? wave_opd(G.wave + tile*RT_WAVE_DOUBLES, R.p1, d0, R.pk, R.dk, R.p, R.d, R.op)
+                                       : CUDART_NAN;
+                if (!WFE || out.opd) out.opd[k] = opd;
+                if (WFE) {
+                    wW = opd;
+                    grid_pupil_coords(G, f, loc, wx, wy);
+                }
+            }
             if (out.abr_x || SUMMARY) {
                 const double rx = G.ref_img ? G.ref_img[tile*2 + 0] : 0.0;
                 const double ry = G.ref_img ? G.ref_img[tile*2 + 1] : 0.0;
@@ -502,6 +596,11 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             cur_tile = tile;
             focus_item(*FP, have, status, fp, fd, op, (int)(tile/G.n_wvls), tile, lc, slice, item, chunk_slots,
                        first, sl, scratch, item_sums);
+        }
+        if (WFE) {
+            const bool first = tile != cur_tile;
+            cur_tile = tile;
+            wfe_item(have, status, wW, wx, wy, tile, first, sl, scratch, item_sums + item*RT_WFE_ITEM_SUMS);
         }
         if (!work_counter) c += gridDim.x;
     }
@@ -555,6 +654,29 @@ k_trace_grid_focus(const rt_surface_desc *__restrict__ g_surfs, const double *__
             const int wi = G.wvl_idx[w];
             trace_ray<false, false>(tab, ntab + (int64_t)wi*n_ifc, g_wvl[wi], n_ifc, o, p0, d0, fw, R);
         }, &F);
+}
+
+/* wavefront-error instance of k_trace_grid (per-ray outputs of kind 0, opd optional) */
+template <bool STAGE>
+__global__ void __launch_bounds__(RT_BLOCK)
+k_trace_grid_wfe(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                 int n_ifc, int n_wvl, GridDev G, int64_t chunk_begin, int64_t chunk_end,
+                 rt_opts o, rt_out out, double *__restrict__ scratch, const double *__restrict__ g_wvl,
+                 int pupil_kind, unsigned long long *work_counter, double *item_sums)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    const rt_surface_desc *tab;
+    const double *ntab;
+    stage_table<STAGE>(g_surfs, g_n, n_ifc, n_wvl, smem, tab, ntab);
+    grid_chunk_loop<false, true, false, true, true>(G, chunk_begin, chunk_end, out, scratch, nullptr, work_counter,
+                                                    item_sums,
+        [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0) {
+            Vec3 p0;
+            grid_start_ray<false>(G, pupil_kind, f, loc, p0, d0);
+            FullWriter fw = {nullptr, 0};
+            const int wi = G.wvl_idx[w];
+            trace_ray<false, true>(tab, ntab + (int64_t)wi*n_ifc, g_wvl[wi], n_ifc, o, p0, d0, fw, R);
+        });
 }
 
 /* ---- lean kernels: plan built in shared memory by the CTA (rt_lean.cuh) */
@@ -638,6 +760,31 @@ k_trace_grid_lean_focus(const rt_surface_desc *__restrict__ g_surfs, const doubl
         }, &F);
 }
 
+/* wavefront-error instance of k_trace_grid_lean (per-ray outputs of kind 0, opd optional) */
+template <bool POLY>
+__global__ void __launch_bounds__(RT_BLOCK, POLY ? 2 : RT_LEAN_MIN_CTAS)
+k_trace_grid_lean_wfe(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                      int n_ifc, int n_wvl, GridDev G, int64_t chunk_begin, int64_t chunk_end,
+                      rt_opts o, rt_out out, double *__restrict__ scratch, unsigned long long *work_counter,
+                      double *item_sums)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    LeanSurf *ls = reinterpret_cast<LeanSurf *>(smem);
+    LeanIdx *li = reinterpret_cast<LeanIdx *>(ls + n_ifc);
+    LeanPoly *lp = reinterpret_cast<LeanPoly *>(li + (size_t)n_ifc*n_wvl);      /* POLY instances only */
+    build_plan(g_surfs, g_n, n_ifc, n_wvl, o, ls, li);
+    if (POLY) build_poly_plan(g_surfs, n_ifc, lp);
+    __syncthreads();
+    grid_chunk_loop<false, true, false, false, true>(G, chunk_begin, chunk_end, out, scratch, nullptr, work_counter,
+                                                     item_sums,
+        [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0) {
+            Vec3 p0;
+            grid_start_ray<true>(G, RT_PUPIL_EPD, f, loc, p0, d0);
+            FullWriter fw = {nullptr, 0};
+            trace_ray_lean<0, true, POLY>(ls, li + (int64_t)G.wvl_idx[w]*n_ifc, lp, g_surfs, n_ifc, o, p0, d0, fw, R);
+        });
+}
+
 /* division self-test: div_shared/normalize3_shared against the IEEE `/` */
 __global__ void k_selftest_division(uint64_t seed, int64_t n_per_thread, unsigned long long *mismatch)
 {
@@ -700,41 +847,66 @@ __global__ void k_selftest_division(uint64_t seed, int64_t n_per_thread, unsigne
  * CTA that finishes last (ticket) combines the RT_RED_SPLIT partials in order. */
 #define RT_RED_THREADS 256
 #define RT_RED_SPLIT 16
+
+/* Record layouts of the reductions.  A record holds ACC accumulated columns, then (in scratch
+ * records) a valid flag at column ACC; W doubles per record and per summary row.  SH: row stride
+ * of reduce_tile's shared-memory tree. */
+struct SpotLayout {        /* RT_SUMMARY_DOUBLES: spot sums */
+    static constexpr int W = RT_SUMMARY_DOUBLES, ACC = RT_ACC, N_ITEM = RT_ITEM_SUMS, SH = RT_SUMMARY_DOUBLES + 1;
+    static __device__ __forceinline__ constexpr bool is_min(int k) { return k == 10 || k == 12; }
+    static __device__ __forceinline__ constexpr bool is_max(int k) { return k == 11 || k == 13; }
+    /* column of per-item sum j: sum_x, sum_y, sum_xx, sum_yy, sum_xy, sum_op */
+    static __device__ __forceinline__ constexpr int item_col(int j) { return j < 5 ? 5 + j : 14; }
+};
+struct WfeLayout {         /* RT_WFE_DOUBLES: wavefront-error sums */
+    static constexpr int W = RT_WFE_DOUBLES, ACC = 20, N_ITEM = RT_WFE_ITEM_SUMS, SH = 21;
+    static __device__ __forceinline__ constexpr bool is_min(int k) { return k == 5; }
+    static __device__ __forceinline__ constexpr bool is_max(int k) { return k == 6; }
+    static __device__ __forceinline__ constexpr int item_col(int j) { return 7 + j; }
+};
+
+template <typename L>
 __device__ __forceinline__ double red_op(int k, double a, double y)
 {
-    if (k == 10 || k == 12) return fmin(a, y);
-    if (k == 11 || k == 13) return fmax(a, y);
+    if (L::is_min(k)) return fmin(a, y);
+    if (L::is_max(k)) return fmax(a, y);
     return a + y;
 }
 
-/* body of k_reduce_summary.  FOCUS: the summary tiles are n planes x n_tiles grid tiles
- * (plane-major) and plane k's per-item sums start at item_sums + k*plane_items*RT_ITEM_SUMS */
-template <bool FOCUS>
+template <typename L>
+__device__ __forceinline__ double red_identity(int k)
+{
+    return L::is_min(k) ? CUDART_INF : (L::is_max(k) ? -CUDART_INF : 0.0);
+}
+
+/* body of k_reduce_summary / k_reduce_wfe for the records of layout L.  FOCUS: the summary tiles
+ * are n planes x n_tiles grid tiles (plane-major) and plane k's per-item sums start at
+ * item_sums + k*plane_items*L::N_ITEM */
+template <typename L, bool FOCUS>
 __device__ __forceinline__ void reduce_tile(const double *__restrict__ scratch, int64_t recs_per_tile,
                                             double *partials, unsigned int *tickets,
                                             double *__restrict__ summary, const double *__restrict__ item_sums,
                                             int64_t chunk_begin, int64_t chunk_end, int64_t chunks_per_tile,
                                             int64_t n_tiles, int64_t plane_items)
 {
-    __shared__ double sh[RT_RED_THREADS][RT_SUMMARY_DOUBLES + 1];
+    __shared__ double sh[RT_RED_THREADS][L::SH];
     __shared__ bool last;
     const int64_t tile = blockIdx.x/RT_RED_SPLIT;
     const int part = blockIdx.x%RT_RED_SPLIT;
     const int64_t plane = FOCUS ? tile/n_tiles : 0;
     const int64_t gtile = FOCUS ? tile - plane*n_tiles : tile;     /* the grid tile whose chunks it covers */
-    if (FOCUS && item_sums) item_sums += plane*plane_items*RT_ITEM_SUMS;
+    if (FOCUS && item_sums) item_sums += plane*plane_items*L::N_ITEM;
     const int64_t per = (recs_per_tile + RT_RED_SPLIT - 1)/RT_RED_SPLIT;
     int64_t r0 = part*per, r1 = r0 + per;
     if (r1 > recs_per_tile) r1 = recs_per_tile;
-    double x[RT_ACC];
+    double x[L::ACC];
 #pragma unroll
-    for (int k = 0; k < RT_ACC; k++)
-        x[k] = (k == 10 || k == 12) ? CUDART_INF : ((k == 11 || k == 13) ? -CUDART_INF : 0.0);
+    for (int k = 0; k < L::ACC; k++) x[k] = red_identity<L>(k);
     for (int64_t r = r0 + threadIdx.x; r < r1; r += RT_RED_THREADS) {
-        const double *p = scratch + (tile*recs_per_tile + r)*RT_SUMMARY_DOUBLES;
-        if (p[RT_ACC] != 0.0) {
+        const double *p = scratch + (tile*recs_per_tile + r)*L::W;
+        if (p[L::ACC] != 0.0) {
 #pragma unroll
-            for (int k = 0; k < RT_ACC; k++) x[k] = red_op(k, x[k], p[k]);
+            for (int k = 0; k < L::ACC; k++) x[k] = red_op<L>(k, x[k], p[k]);
         }
     }
     if (item_sums) {
@@ -748,41 +920,43 @@ __device__ __forceinline__ void reduce_tile(const double *__restrict__ scratch, 
             const int64_t per_it = (n_it + RT_RED_SPLIT - 1)/RT_RED_SPLIT;
             int64_t a0 = part*per_it, a1 = a0 + per_it;
             if (a1 > n_it) a1 = n_it;
-            const int col[RT_ITEM_SUMS] = {5, 6, 7, 8, 9, 14};
-            for (int64_t it = a0 + threadIdx.x; it < a1; it += RT_RED_THREADS) {
-                const double *p = item_sums + (i0 + it)*RT_ITEM_SUMS;
+            int col[L::N_ITEM];
 #pragma unroll
-                for (int k = 0; k < RT_ITEM_SUMS; k++) x[col[k]] += p[k];
+            for (int k = 0; k < L::N_ITEM; k++) col[k] = L::item_col(k);
+            for (int64_t it = a0 + threadIdx.x; it < a1; it += RT_RED_THREADS) {
+                const double *p = item_sums + (i0 + it)*L::N_ITEM;
+#pragma unroll
+                for (int k = 0; k < L::N_ITEM; k++) x[col[k]] += p[k];
             }
         }
     }
 #pragma unroll
-    for (int k = 0; k < RT_ACC; k++) sh[threadIdx.x][k] = x[k];
+    for (int k = 0; k < L::ACC; k++) sh[threadIdx.x][k] = x[k];
     __syncthreads();
     for (int off = RT_RED_THREADS/2; off > 0; off >>= 1) {
         if (threadIdx.x < off) {
 #pragma unroll
-            for (int k = 0; k < RT_ACC; k++)
-                sh[threadIdx.x][k] = red_op(k, sh[threadIdx.x][k], sh[threadIdx.x + off][k]);
+            for (int k = 0; k < L::ACC; k++)
+                sh[threadIdx.x][k] = red_op<L>(k, sh[threadIdx.x][k], sh[threadIdx.x + off][k]);
         }
         __syncthreads();
     }
-    double *mine = partials + ((int64_t)blockIdx.x)*RT_SUMMARY_DOUBLES;
-    if (threadIdx.x < RT_ACC) mine[threadIdx.x] = sh[0][threadIdx.x];
+    double *mine = partials + ((int64_t)blockIdx.x)*L::W;
+    if (threadIdx.x < L::ACC) mine[threadIdx.x] = sh[0][threadIdx.x];
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) last = (atomicAdd(&tickets[tile], 1u) == RT_RED_SPLIT - 1);
     __syncthreads();
-    if (last && threadIdx.x < RT_SUMMARY_DOUBLES) {
+    if (last && threadIdx.x < L::W) {
         __threadfence();
         const int k = threadIdx.x;
         double v = 0.0;
-        if (k < RT_ACC) {
-            const volatile double *pp = partials + tile*RT_RED_SPLIT*RT_SUMMARY_DOUBLES;
+        if (k < L::ACC) {
+            const volatile double *pp = partials + tile*RT_RED_SPLIT*L::W;
             v = pp[k];
-            for (int j = 1; j < RT_RED_SPLIT; j++) v = red_op(k, v, pp[j*RT_SUMMARY_DOUBLES + k]);
+            for (int j = 1; j < RT_RED_SPLIT; j++) v = red_op<L>(k, v, pp[j*L::W + k]);
         }
-        summary[tile*RT_SUMMARY_DOUBLES + k] = v;
+        summary[tile*L::W + k] = v;
     }
 }
 
@@ -792,8 +966,8 @@ k_reduce_summary(const double *__restrict__ scratch, int64_t recs_per_tile, doub
                  const double *__restrict__ item_sums, int64_t chunk_begin, int64_t chunk_end,
                  int64_t chunks_per_tile)
 {
-    reduce_tile<false>(scratch, recs_per_tile, partials, tickets, summary, item_sums, chunk_begin, chunk_end,
-                       chunks_per_tile, 0, 0);
+    reduce_tile<SpotLayout, false>(scratch, recs_per_tile, partials, tickets, summary, item_sums, chunk_begin,
+                                   chunk_end, chunks_per_tile, 0, 0);
 }
 
 /* k_reduce_summary over the n planes x n_tiles summary tiles of rt_trace_grid_focus */
@@ -803,8 +977,19 @@ k_reduce_summary_focus(const double *__restrict__ scratch, int64_t recs_per_tile
                        const double *__restrict__ item_sums, int64_t chunk_begin, int64_t chunk_end,
                        int64_t chunks_per_tile, int64_t n_tiles, int64_t plane_items)
 {
-    reduce_tile<true>(scratch, recs_per_tile, partials, tickets, summary, item_sums, chunk_begin, chunk_end,
-                      chunks_per_tile, n_tiles, plane_items);
+    reduce_tile<SpotLayout, true>(scratch, recs_per_tile, partials, tickets, summary, item_sums, chunk_begin,
+                                  chunk_end, chunks_per_tile, n_tiles, plane_items);
+}
+
+/* k_reduce_summary for the wavefront-error records and item sums of rt_trace_grid_wfe */
+__global__ void __launch_bounds__(RT_RED_THREADS)
+k_reduce_wfe(const double *__restrict__ scratch, int64_t recs_per_tile, double *partials,
+             unsigned int *tickets, double *__restrict__ summary,
+             const double *__restrict__ item_sums, int64_t chunk_begin, int64_t chunk_end,
+             int64_t chunks_per_tile)
+{
+    reduce_tile<WfeLayout, false>(scratch, recs_per_tile, partials, tickets, summary, item_sums, chunk_begin,
+                                  chunk_end, chunks_per_tile, 0, 0);
 }
 
 /* summary of an empty chunk range: zero counts / sums, identities in the min / max columns */
@@ -816,16 +1001,36 @@ __global__ void k_summary_identity(double *__restrict__ summary, int64_t n)
     summary[i] = (k == 10 || k == 12) ? CUDART_INF : ((k == 11 || k == 13) ? -CUDART_INF : 0.0);
 }
 
-/* out[tile][k] = parts[0][tile][k] (+|min|max) parts[1][tile][k] ... in part order */
-__global__ void k_combine_summaries(const double *__restrict__ parts, int n_parts, int64_t n,
-                                    double *__restrict__ out)
+/* k_summary_identity for wavefront-error records */
+__global__ void k_wfe_identity(double *__restrict__ summary, int64_t n)
 {
     const int64_t i = (int64_t)blockIdx.x*blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int k = (int)(i % RT_SUMMARY_DOUBLES);
+    summary[i] = red_identity<WfeLayout>((int)(i % RT_WFE_DOUBLES));
+}
+
+/* out[tile][k] = parts[0][tile][k] (+|min|max) parts[1][tile][k] ... in part order */
+template <typename L>
+__device__ __forceinline__ void combine_rows(const double *__restrict__ parts, int n_parts, int64_t n,
+                                             double *__restrict__ out)
+{
+    const int64_t i = (int64_t)blockIdx.x*blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int k = (int)(i % L::W);
     double v = parts[i];
-    for (int p = 1; p < n_parts; p++) v = red_op(k, v, parts[(int64_t)p*n + i]);
+    for (int p = 1; p < n_parts; p++) v = red_op<L>(k, v, parts[(int64_t)p*n + i]);
     out[i] = v;
+}
+
+__global__ void k_combine_summaries(const double *__restrict__ parts, int n_parts, int64_t n,
+                                    double *__restrict__ out)
+{
+    combine_rows<SpotLayout>(parts, n_parts, n, out);
+}
+
+__global__ void k_combine_wfe(const double *__restrict__ parts, int n_parts, int64_t n, double *__restrict__ out)
+{
+    combine_rows<WfeLayout>(parts, n_parts, n, out);
 }
 
 /* chief rays of all fields: pupil (0, 0), no vignetting, apertures not checked, general
@@ -1080,7 +1285,7 @@ static int single_focus_grid(const rt_table *t, const rt_grid *g, int64_t cb, in
 }
 
 template <typename K, typename... Args>
-static int launch_focus_kernel(K kern, size_t smem, const rt_table *t, const rt_grid *g, int64_t cb, int64_t ce,
+static int launch_item_kernel(K kern, size_t smem, const rt_table *t, const rt_grid *g, int64_t cb, int64_t ce,
                                bool chunk_slots, cudaStream_t stream, Args... args)
 {
     int rc = prep_kernel(kern, smem);
@@ -1646,12 +1851,12 @@ int rt_trace_grid_focus(const rt_table *t, const rt_grid *g, int64_t chunk_begin
     /* angular pupil specifications are generated by the general kernels only (rt_grid.cuh) */
     if (t->lean && g->pupil_kind == RT_PUPIL_EPD) {
         auto kern = t->lean_poly ? k_trace_grid_lean_focus<true> : k_trace_grid_lean_focus<false>;
-        rc = launch_focus_kernel(kern, t->lean_bytes, t, g, chunk_begin, chunk_end, chunk_slots, s,
+        rc = launch_item_kernel(kern, t->lean_bytes, t, g, chunk_begin, chunk_end, chunk_slots, s,
                                  t->d_surfs, t->d_n, t->n_ifc, t->n_wvl, G, chunk_begin, chunk_end, *o, *out,
                                  scr, wc, items, P, L);
     } else {
         auto kern = t->stage ? k_trace_grid_focus<true> : k_trace_grid_focus<false>;
-        rc = launch_focus_kernel(kern, t->stage ? t->stage_bytes : 0, t, g, chunk_begin, chunk_end, chunk_slots, s,
+        rc = launch_item_kernel(kern, t->stage ? t->stage_bytes : 0, t, g, chunk_begin, chunk_end, chunk_slots, s,
                                  t->d_surfs, t->d_n, t->n_ifc, t->n_wvl, G, chunk_begin, chunk_end, *o, *out,
                                  scr, t->d_wvl, g->pupil_kind, wc, items, P, L);
     }
@@ -1671,6 +1876,88 @@ int rt_combine_summaries(const double *parts, int32_t n_parts, int64_t n_tiles, 
     if (n_tiles == 0) return RT_OK;
     const int64_t n = n_tiles*RT_SUMMARY_DOUBLES;
     k_combine_summaries<<<(unsigned)((n + 255)/256), 256, 0, (cudaStream_t)stream>>>(parts, n_parts, n, out);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+/* scratch of rt_trace_grid_wfe: records [n_tiles][slots][RT_WARPS][RT_WFE_DOUBLES] | partials
+ * [n_tiles][RT_RED_SPLIT][RT_WFE_DOUBLES] | tickets [n_tiles] | per-item sums [items][RT_WFE_ITEM_SUMS] */
+static int64_t wfe_head_doubles(const rt_grid *g)
+{
+    return (scratch_records(g) + g->n_tiles*RT_RED_SPLIT)*RT_WFE_DOUBLES + g->n_tiles;
+}
+
+int64_t rt_grid_wfe_scratch_bytes(const rt_grid *g, int64_t chunk_begin, int64_t chunk_end)
+{
+    if (!g || chunk_end < chunk_begin) return 0;
+    return (wfe_head_doubles(g) + (chunk_end - chunk_begin)*RT_WARPS*RT_WFE_ITEM_SUMS)*(int64_t)sizeof(double);
+}
+
+int rt_trace_grid_wfe(const rt_table *t, const rt_grid *g, int64_t chunk_begin, int64_t chunk_end,
+                      const rt_opts *o, const rt_out *out, double *summary, void *scratch, void *stream)
+{
+    if (!t || !g || !out) return fail(RT_ERR_INVALID, "rt_trace_grid_wfe: bad arguments");
+    if (!summary || !scratch) return fail(RT_ERR_INVALID, "rt_trace_grid_wfe: summary and scratch are required");
+    if (out->full) return fail(RT_ERR_INVALID, "rt_trace_grid_wfe: full must be NULL");
+    if (!g->d_wave) return fail(RT_ERR_INVALID, "rt_trace_grid_wfe: the grid has no wave records (rt_grid_spec.wave)");
+    if (t->device != g->device) return fail(RT_ERR_INVALID, "rt_trace_grid_wfe: table and grid on different devices");
+    if (chunk_begin < 0 || chunk_end > g->n_chunks || chunk_end < chunk_begin)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_wfe: chunk range out of bounds");
+    int rc = check_opts(t, o);
+    if (rc) return rc;
+    for (int32_t wi : g->h_wvl_idx)
+        if (wi < 0 || wi >= t->n_wvl)
+            return fail(RT_ERR_INVALID, "rt_trace_grid_wfe: the grid's wvl_idx is out of range for this table");
+    if (out_kind(out) != 0) return fail(RT_ERR_UNSUPPORTED, "rt_trace_grid_wfe: opd cannot be combined with normals");
+    if (!t->wave_ok)
+        return fail(RT_ERR_UNSUPPORTED, "rt_trace_grid_wfe: opd needs >= 3 interfaces and no decenter on the last one before the image");
+    DeviceGuard guard(t->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (chunk_begin == chunk_end) {
+        const int64_t n = g->n_tiles*RT_WFE_DOUBLES;
+        k_wfe_identity<<<(unsigned)((n + 255)/256), 256, 0, s>>>(summary, n);
+        g_launches++;
+        CUDA_TRY(cudaGetLastError());
+        return RT_OK;
+    }
+    double *scr = (double *)scratch;
+    const int64_t recs = scratch_records(g);
+    double *partials = scr + recs*RT_WFE_DOUBLES;
+    unsigned int *tickets = (unsigned int *)(partials + g->n_tiles*RT_RED_SPLIT*RT_WFE_DOUBLES);
+    double *items = scr + wfe_head_doubles(g);
+    /* the per-item sums are all written by the trace: zero the records, partials and tickets only */
+    CUDA_TRY(cudaMemsetAsync(scr, 0, (size_t)wfe_head_doubles(g)*sizeof(double), s));
+    unsigned long long *wc;
+    if ((rc = launch_counter(t, s, &wc, true))) return rc;
+    const GridDev G = grid_dev(g);
+    /* the kernel family rt_trace_grid takes for an opd launch; angular pupil specifications are
+     * generated by the general kernels only (rt_grid.cuh) */
+    if (t->lean && g->pupil_kind == RT_PUPIL_EPD) {
+        auto kern = t->lean_poly ? k_trace_grid_lean_wfe<true> : k_trace_grid_lean_wfe<false>;
+        rc = launch_item_kernel(kern, t->lean_bytes, t, g, chunk_begin, chunk_end, false, s,
+                                t->d_surfs, t->d_n, t->n_ifc, t->n_wvl, G, chunk_begin, chunk_end, *o, *out,
+                                scr, wc, items);
+    } else {
+        auto kern = t->stage ? k_trace_grid_wfe<true> : k_trace_grid_wfe<false>;
+        rc = launch_item_kernel(kern, t->stage ? t->stage_bytes : 0, t, g, chunk_begin, chunk_end, false, s,
+                                t->d_surfs, t->d_n, t->n_ifc, t->n_wvl, G, chunk_begin, chunk_end, *o, *out,
+                                scr, t->d_wvl, g->pupil_kind, wc, items);
+    }
+    if (rc) return rc;
+    k_reduce_wfe<<<(unsigned)(g->n_tiles*RT_RED_SPLIT), RT_RED_THREADS, 0, s>>>(
+        scr, recs/g->n_tiles, partials, tickets, summary, items, chunk_begin, chunk_end, g->chunks_per_tile);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+int rt_combine_wfe(const double *parts, int32_t n_parts, int64_t n_tiles, double *out, void *stream)
+{
+    if (!parts || !out || n_parts < 1 || n_tiles < 0) return fail(RT_ERR_INVALID, "rt_combine_wfe: bad arguments");
+    if (n_tiles == 0) return RT_OK;
+    const int64_t n = n_tiles*RT_WFE_DOUBLES;
+    k_combine_wfe<<<(unsigned)((n + 255)/256), 256, 0, (cudaStream_t)stream>>>(parts, n_parts, n, out);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RT_OK;

@@ -92,4 +92,22 @@ __device__ __forceinline__ void grid_start_ray(const GridDev &G, int pupil_kind,
     grid_start_ray_at<LEAN>(G, pupil_kind, f, pupx, pupy, G.apply_vignetting != 0, p0, d0);
 }
 
+/* relative pupil coordinates of grid ray (tile, loc) as grid_start_ray uses them: pupil_x[i] and
+ * pupil_y[j] (product grid) or pupil_y[i] (ray list) of field f, after Field.apply_vignetting
+ * when the grid applies it */
+__device__ __forceinline__ void grid_pupil_coords(const GridDev &G, int f, int64_t loc, double &pupx, double &pupy)
+{
+    const int i = (int)(loc/G.ny), j = (int)(loc - (int64_t)i*G.ny);
+    pupx = G.pupil_x[(int64_t)f*G.nx + i];
+    pupy = G.paired ? G.pupil_y[(int64_t)f*G.nx + i] : G.pupil_y[(int64_t)f*G.ny + j];
+    if (G.apply_vignetting) {
+        const rt_field_desc &F = G.fields[f];
+        const double vlx = F.vlx, vux = F.vux, vly = F.vly, vuy = F.vuy;
+        if (pupx < 0.0) { if (vlx != 0.0) pupx *= (1.0 - vlx); }
+        else            { if (vux != 0.0) pupx *= (1.0 - vux); }
+        if (pupy < 0.0) { if (vly != 0.0) pupy *= (1.0 - vly); }
+        else            { if (vuy != 0.0) pupy *= (1.0 - vuy); }
+    }
+}
+
 }  // namespace b200rt

@@ -19,11 +19,19 @@ import numpy as np
 import torch
 
 from . import _abi
-from ._abi import rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES
+from ._abi import rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES, RT_WFE_DOUBLES
 
 SUMMARY_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other',
                   'sum_x', 'sum_y', 'sum_xx', 'sum_yy', 'sum_xy',
                   'min_x', 'max_x', 'min_y', 'max_y', 'sum_op', 'reserved')
+# columns of a wavefront-error record (RT_WFE_DOUBLES, include/b200rt.h): W = OPD in system units,
+# (x, y) relative pupil coordinates, r2 = x*x + y*y
+WFE_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other', 'min_w', 'max_w',
+              'sum_w', 'sum_ww', 'sum_xw', 'sum_yw', 'sum_r2w',
+              'sum_x', 'sum_y', 'sum_xx', 'sum_xy', 'sum_yy', 'sum_xr2', 'sum_yr2', 'sum_r2r2',
+              'reserved0', 'reserved1', 'reserved2', 'reserved3')
+# min / max columns of the two record layouts, by record width
+_MINMAX_COLS = {RT_SUMMARY_DOUBLES: ((10, 12), (11, 13)), RT_WFE_DOUBLES: ((5,), (6,))}
 
 
 def _ptr(t):
@@ -487,23 +495,30 @@ def decode_nan_status(abr):
 
 
 def combine_summaries(parts, out=None):
-    """Combine partial ``[n_tiles, 16]`` summaries (from chunk ranges / ranks):
-    sums add, min/max columns take min/max.  CUDA tensors: one ``rt_combine_summaries``
-    launch on the current stream; CPU tensors (gloo tests): torch."""
+    """Combine partial ``[n_tiles, 16]`` spot summaries or ``[n_tiles, RT_WFE_DOUBLES]``
+    wavefront-error records (from chunk ranges / ranks; the layout is chosen by ``shape[-1]``):
+    sums add in part order, min/max columns take min/max.  CUDA tensors: one
+    ``rt_combine_summaries`` / ``rt_combine_wfe`` launch on the current stream; CPU tensors (gloo
+    tests): torch."""
     parts = torch.stack(list(parts)) if not torch.is_tensor(parts) else parts
+    width = parts.shape[-1]
+    if width not in _MINMAX_COLS:
+        raise ValueError(f'unknown summary width {width}')
     if parts.is_cuda:
         parts = parts.contiguous()
         if out is None:
             out = torch.empty(parts.shape[1:], dtype=parts.dtype, device=parts.device)
+        lib = _abi.load_library()
+        fn = lib.rt_combine_summaries if width == RT_SUMMARY_DOUBLES else lib.rt_combine_wfe
         with torch.cuda.device(parts.device):
-            _abi.check(_abi.load_library().rt_combine_summaries(
-                _ptr(parts), parts.shape[0], parts.shape[1], _ptr(out), _stream_ptr(parts.device)))
+            _abi.check(fn(_ptr(parts), parts.shape[0], parts.shape[1], _ptr(out), _stream_ptr(parts.device)))
         out._keep = parts
         return out
     out = parts.sum(dim=0)
-    for k in (10, 12):
+    mins, maxs = _MINMAX_COLS[width]
+    for k in mins:
         out[:, k] = parts[:, :, k].min(dim=0).values
-    for k in (11, 13):
+    for k in maxs:
         out[:, k] = parts[:, :, k].max(dim=0).values
     return out
 
@@ -524,6 +539,101 @@ def spot_statistics(summary):
             'centroid_x': cx, 'centroid_y': cy, 'rms_radius': sqrt0(var),
             'min_x': s[:, 10], 'max_x': s[:, 11], 'min_y': s[:, 12], 'max_y': s[:, 13],
             'mean_op': s[:, 14]/n}
+
+
+def trace_grid_wfe(table, grid, chunk_begin=0, chunk_end=None, res=None, **kwargs):
+    """Wavefront-error sums of chunks ``[chunk_begin, chunk_end)`` of a PupilGrid built with
+    ``wave=`` records (``rt_trace_grid_wfe``): ``[n_tiles, RT_WFE_DOUBLES]`` float64 device tensor
+    (WFE_FIELDS; ``wavefront_statistics`` turns it into numbers).  ``res``: optional BundleResult
+    that receives per-ray outputs as ``trace_grid`` writes them (``opd`` included; no whole rays).
+    Trace defaults as ``trace_grid``.  Asynchronous on the current CUDA stream."""
+    lib = _abi.load_library()
+    device = torch.device('cuda', table.device)
+    if chunk_end is None:
+        chunk_end = grid.n_chunks
+    kwargs.setdefault('check_apertures', True)
+    kwargs.setdefault('first_surf', 1)
+    kwargs.setdefault('last_surf', table.n_ifc - 2)
+    if grid.pupil_kind == _abi.PUPIL_WIDE:
+        kwargs['intersect_obj'] = False
+    opts = _abi.make_opts(**kwargs)
+    if res is None:
+        res = BundleResult(0, table.n_ifc, device, ())
+    elif res.n != grid.rays_in_chunks(chunk_begin, chunk_end):
+        raise ValueError('res was allocated for a different number of rays')
+    out = res.c_struct()
+    summ = torch.empty((grid.n_tiles, RT_WFE_DOUBLES), dtype=torch.float64, device=device)
+    nbytes = lib.rt_grid_wfe_scratch_bytes(grid.handle, chunk_begin, chunk_end)
+    scratch = torch.empty(max(nbytes//8, 1), dtype=torch.float64, device=device)
+    _abi.check(lib.rt_trace_grid_wfe(table.handle, grid.handle, chunk_begin, chunk_end, C.byref(opts),
+                                     C.byref(out), _ptr(summ), _ptr(scratch), _stream_ptr(device)))
+    summ._keep = scratch          # scratch must outlive the asynchronous launches
+    return summ
+
+
+WFE_STATISTICS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other', 'rms', 'pv', 'rms_tilt', 'tilt_x',
+                  'tilt_y', 'rms_focus', 'focus')
+
+
+def _fit(gram, rhs, sum_ww, n):
+    """Least-squares fit from the normal equations of one tile: ``(coefficients, RSS)``; NaN
+    when there are fewer rays than basis functions or the Gram matrix is rank deficient"""
+    p = len(rhs)
+    nan = (np.full(p, np.nan), np.nan)
+    if not (n >= p) or not np.isfinite(gram).all() or not np.isfinite(rhs).all():
+        return nan
+    d = np.sqrt(np.diag(gram))
+    if not (d > 0).all():
+        return nan
+    scaled = gram/np.outer(d, d)             # unit diagonal: its condition number is the fit's
+    ev = np.linalg.eigvalsh(scaled)
+    if not ev[0] > p*np.finfo(np.float64).eps*ev[-1]:
+        return nan
+    c = np.linalg.solve(scaled, rhs/d)/d
+    return c, sum_ww - float(np.dot(c, rhs))
+
+
+def wavefront_statistics(summary, wvl_sys):
+    """Per-tile wavefront error from combined ``[n_tiles, RT_WFE_DOUBLES]`` records (numpy array
+    or torch tensor; same type out, on the same device).  ``wvl_sys``: the wavelength in system
+    units (``opt_model.nm_to_sys_units(wvl)``), a scalar or one value per tile; every result is
+    in waves.
+
+    ``rms``: sqrt(sum W^2/n - (sum W/n)^2), piston removed; ``pv``: max W - min W;
+    ``rms_tilt``, ``tilt_x``, ``tilt_y``: least-squares fit of W on {1, x, y}, its residual
+    sqrt(RSS/n) with RSS = sum W^2 - c.b from the 3 x 3 normal equations; ``rms_focus``,
+    ``focus``: the same on {1, x, y, r^2} (4 x 4).  Coefficients are in waves at unit relative
+    pupil.  A fit with fewer rays than basis functions or a rank-deficient Gram matrix is NaN;
+    a tile without a status-0 ray is NaN everywhere except the counts."""
+    is_t = torch.is_tensor(summary)
+    s = (summary.detach().cpu().numpy() if is_t else np.asarray(summary, dtype=np.float64)).reshape(-1, RT_WFE_DOUBLES)
+    lam = np.broadcast_to(np.asarray(wvl_sys, dtype=np.float64).reshape(-1), (s.shape[0],))
+    n = s[:, 0]
+    out = {k: s[:, i].copy() for i, k in enumerate(WFE_STATISTICS[:5])}
+    for k in WFE_STATISTICS[5:]:
+        out[k] = np.full(s.shape[0], np.nan)
+    for t in range(s.shape[0]):
+        (nt, sw, sww, sxw, syw, sr2w, sx, sy, sxx, sxy, syy, sxr2, syr2, sr2r2) = \
+            (s[t, 0],) + tuple(s[t, 7:20])
+        if not nt > 0:
+            continue
+        lt = lam[t]
+        with np.errstate(invalid='ignore'):
+            mean = sw/nt
+            out['rms'][t] = np.sqrt(max(sww/nt - mean*mean, 0.0))/lt if np.isfinite(sww) else np.nan
+        out['pv'][t] = (s[t, 6] - s[t, 5])/lt
+        sr2 = sxx + syy
+        g3 = np.array([[nt, sx, sy], [sx, sxx, sxy], [sy, sxy, syy]])
+        c3, rss3 = _fit(g3, np.array([sw, sxw, syw]), sww, nt)
+        out['rms_tilt'][t] = np.sqrt(max(rss3, 0.0)/nt)/lt if np.isfinite(rss3) else np.nan
+        out['tilt_x'][t], out['tilt_y'][t] = c3[1]/lt, c3[2]/lt
+        g4 = np.array([[nt, sx, sy, sr2], [sx, sxx, sxy, sxr2], [sy, sxy, syy, syr2], [sr2, sxr2, syr2, sr2r2]])
+        c4, rss4 = _fit(g4, np.array([sw, sxw, syw, sr2w]), sww, nt)
+        out['rms_focus'][t] = np.sqrt(max(rss4, 0.0)/nt)/lt if np.isfinite(rss4) else np.nan
+        out['focus'][t] = c4[3]/lt
+    if is_t:
+        return {k: torch.as_tensor(v, device=summary.device) for k, v in out.items()}
+    return out
 
 
 def measure_fp64_peak(device=0):
