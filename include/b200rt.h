@@ -44,6 +44,8 @@ extern "C" {
 #define RT_WAVE_DOUBLES 24   /* per-(field, wvl) chief-ray / reference-sphere record, see rt_grid_spec.wave */
 #define RT_MAX_FOCUS 64      /* image planes of one rt_trace_grid_focus call */
 #define RT_WFE_DOUBLES 24    /* per-tile wavefront-error record of rt_trace_grid_wfe */
+#define RT_ZERN_DOUBLES 752  /* per-tile Zernike moments record of rt_grid_zernike */
+#define RT_ZERN_MAX_TERMS 37 /* Fringe Zernike terms of rt_grid_zernike */
 
 /* error codes (function return values) */
 enum rt_error {
@@ -390,6 +392,34 @@ int rt_trace_grid_wfe(const rt_table *table, const rt_grid *grid,
  * -> out DEVICE [n_tiles][RT_WFE_DOUBLES]; sums and counts add in part order, column 5 takes fmin,
  * column 6 fmax.  One launch on `stream`. */
 int rt_combine_wfe(const double *parts, int32_t n_parts, int64_t n_tiles, double *out, void *stream);
+
+/* ---- Zernike moments (ABI 6, additive): the packed Gram matrix of a = [W, Z_1 ... Z_J] per tile,
+ * the normal equations of a least-squares fit of the OPD on the first J Fringe Zernike terms
+ * (csrc/rt_zernike.cuh).  status / opd: DEVICE per-ray arrays indexed as rt_trace_grid's outputs
+ * over the same chunk range (rays_in_chunks(chunk_begin, chunk_end) entries; opd in system units).
+ * (x, y) = the ray's relative pupil coordinates pupil_x[i], pupil_y[j] of its rt_grid_spec.  A ray
+ * is used when its status is 0 and x*x + y*y <= 1.  summary: DEVICE [n_tiles][RT_ZERN_DOUBLES]:
+ *   0-4 status-class counts of every ray (as the wavefront-error record)   5 n_used
+ *   6 min W 7 max W over the used rays (fmin / fmax: NaN skipped; +-inf without used rays)   8 0
+ *   9 + j*(j+1)/2 + i, i <= j <= J: sum of a_i*a_j over the used rays (a_0 = W, a_k = Z_k)
+ *   later columns 0
+ * Sum order (DESIGN.md section 4): products rounded once; per chunk of 256 rays of one tile every
+ * entry is added in ray order from +0.0; the tile's chunk sums inside the range are added in chunk
+ * order from +0.0.  Bit-reproducible, independent of the launch shape. */
+/* DEVICE scratch bytes of rt_grid_zernike over [chunk_begin, chunk_end) with n_terms terms;
+ * 0 for bad arguments or an empty range */
+int64_t rt_grid_zernike_scratch_bytes(const rt_grid *grid, int64_t chunk_begin, int64_t chunk_end,
+                                      int32_t n_terms);
+/* The grid must be a product grid (paired = 0) without apply_vignetting; 1 <= n_terms <=
+ * RT_ZERN_MAX_TERMS.  status, opd and scratch may be NULL only for an empty range; summary is
+ * required.  RT_ERR_INVALID before any device work for bad arguments.  Two kernel launches (the
+ * moments, their reduction), one for an empty chunk range. */
+int rt_grid_zernike(const rt_grid *grid, int64_t chunk_begin, int64_t chunk_end, int32_t n_terms,
+                    const int32_t *status, const double *opd, double *summary, void *scratch, void *stream);
+/* rt_combine_summaries for Zernike moments records: parts DEVICE [n_parts][n_tiles][RT_ZERN_DOUBLES]
+ * -> out DEVICE [n_tiles][RT_ZERN_DOUBLES]; sums and counts add in part order, column 6 takes fmin,
+ * column 7 fmax.  One launch on `stream`. */
+int rt_combine_zernike(const double *parts, int32_t n_parts, int64_t n_tiles, double *out, void *stream);
 
 /* ---- misc */
 const char *rt_last_error(void);

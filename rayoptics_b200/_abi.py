@@ -18,6 +18,8 @@ RT_SUMMARY_DOUBLES = 16
 RT_WAVE_DOUBLES = 24
 RT_MAX_FOCUS = 64
 RT_WFE_DOUBLES = 24
+RT_ZERN_DOUBLES = 752
+RT_ZERN_MAX_TERMS = 37
 
 # enum rt_profile
 PROFILE_IDS = {'Spherical': 0, 'Conic': 1, 'EvenPolynomial': 2,
@@ -119,7 +121,8 @@ EXPORTS = ['rt_table_create', 'rt_table_destroy', 'rt_table_dims', 'rt_table_set
            'rt_grid_update', 'rt_trace_grid_to_host', 'rt_trace_grid_to_host_scratch_bytes',
            'rt_last_error', 'rt_abi_version', 'rt_chunk_rays', 'rt_launch_count', 'rt_measure_fp64_peak', 'rt_measure_fp64_latency',
            'rt_selftest_division', 'rt_grid_chief_ref_focus', 'rt_grid_focus_scratch_bytes',
-           'rt_trace_grid_focus', 'rt_grid_wfe_scratch_bytes', 'rt_trace_grid_wfe', 'rt_combine_wfe']
+           'rt_trace_grid_focus', 'rt_grid_wfe_scratch_bytes', 'rt_trace_grid_wfe', 'rt_combine_wfe',
+           'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike']
 
 _lib = None
 
@@ -187,6 +190,12 @@ def load_library():
     lib.rt_trace_grid_wfe.restype = i32
     lib.rt_combine_wfe.argtypes = [vp, i32, i64, vp, vp]
     lib.rt_combine_wfe.restype = i32
+    lib.rt_grid_zernike_scratch_bytes.argtypes = [vp, i64, i64, i32]
+    lib.rt_grid_zernike_scratch_bytes.restype = i64
+    lib.rt_grid_zernike.argtypes = [vp, i64, i64, i32, vp, vp, vp, vp, vp]
+    lib.rt_grid_zernike.restype = i32
+    lib.rt_combine_zernike.argtypes = [vp, i32, i64, vp, vp]
+    lib.rt_combine_zernike.restype = i32
     lib.rt_last_error.restype = C.c_char_p
     lib.rt_abi_version.restype = i32
     lib.rt_chunk_rays.restype = i32

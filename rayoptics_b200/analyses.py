@@ -422,6 +422,98 @@ def wavefront_error(opt_model, num_rays=21, fields=None, wvls=None, foc=None, im
     return WavefrontError(stats, summ_host, ref_img, num_rays, len(fields), len(wvls))
 
 
+class ZernikeFit:
+    """Result of ``zernike_fit``: ``coef`` ``[n_fields, n_wvls, num_terms]``, the Fringe Zernike
+    coefficients in waves (``coef[..., 0]`` is Z1, piston); ``[n_fields, n_wvls]`` arrays of
+    ``rms_residual`` (sqrt(RSS/n_used), waves), ``rms`` (piston removed) and ``pv`` over the used
+    rays (waves), ``n_used`` and the ray counts ``n_ok``, ``n_missed``, ``n_tir``, ``n_blocked``,
+    ``n_other`` (``engine.zernike_statistics``).  ``summary``: the combined ``[n_tiles,
+    RT_ZERN_DOUBLES]`` records; ``ref_img`` ``[n_fields, n_wvls, 2]``; ``num_rays``: pupil samples
+    per side; ``num_terms``."""
+
+    def __init__(self, stats, summary, ref_img, num_rays, num_terms, n_fields, n_wvls):
+        self.coef = np.asarray(stats['coef']).reshape(n_fields, n_wvls, num_terms)
+        self.stats = {k: np.asarray(v).reshape(n_fields, n_wvls) for k, v in stats.items() if k != 'coef'}
+        for k, v in self.stats.items():
+            setattr(self, k, v)
+        self.summary, self.ref_img = summary, ref_img
+        self.num_rays, self.num_terms, self.n_fields, self.n_wvls = num_rays, num_terms, n_fields, n_wvls
+
+
+def _zernike_sums_host(spec, status, opd, n_terms):
+    """The ``[n_tiles, RT_ZERN_DOUBLES]`` record of traced rays, formed on the host (the
+    ``backend=`` test seam; the device forms it in ``rt_grid_zernike``)"""
+    from ._abi import RT_ZERN_DOUBLES
+    s = np.zeros((spec.n_tiles, RT_ZERN_DOUBLES))
+    per = spec.rays_per_tile
+    tri = [(i, j) for j in range(n_terms + 1) for i in range(j + 1)]
+    cols = [E.zernike_gram_col(i, j) for i, j in tri]
+    for t in range(spec.n_tiles):
+        f = t//spec.n_wvls
+        gx, gy = np.meshgrid(spec.pupil_x[f], spec.pupil_y[f], indexing='ij')
+        x, y = gx.ravel(), gy.ravel()
+        st, w = status[t*per:(t + 1)*per], opd[t*per:(t + 1)*per]
+        used = (st == 0) & (x*x + y*y <= 1.0)
+        cls = np.where((st >= 0) & (st <= 3), st, 4)
+        s[t, 0:5] = np.bincount(cls, minlength=5)[:5]
+        s[t, 5] = used.sum()
+        s[t, 6] = np.fmin.reduce(w[used], initial=np.inf)
+        s[t, 7] = np.fmax.reduce(w[used], initial=-np.inf)
+        a = np.concatenate([w[used, None], E.zernike_terms(x[used], y[used], n_terms)], axis=1)
+        g = a.T @ a
+        s[t, cols] = [g[i, j] for i, j in tri]
+    return s
+
+
+def zernike_fit(opt_model, num_rays=64, num_terms=37, fields=None, wvls=None, foc=None, image_pt_2d=None,
+                image_delta=None, table=None, device=0, shard=None, group=None, chunk_range=None,
+                backend=None, **kwargs):
+    """Fringe Zernike coefficients of the wavefront of every field and wavelength, from one grid
+    trace.
+
+    The rays are those of ``wavefront_error`` (``RayGrid``'s: a square grid over the field's
+    vignetting bounding box, no vignetting applied, apertures checked, the same chief ray and
+    reference sphere).  The fit is over the unit disk of relative pupil coordinates, restricted to
+    the rays that arrive: a ray is used when its status is 0 and x^2 + y^2 <= 1.  The OPDs are
+    reduced on the device to the Gram matrix of [W, Z_1 ... Z_num_terms] per tile
+    (``rt_grid_zernike``) and only that comes back; the normal equations are solved on the host
+    (``engine.zernike_statistics``).  ``num_terms``: 1 ... 37, the first Fringe terms.
+    ``shard=(rank, world)`` / ``group`` / ``chunk_range`` as ``spot_diagram``: one all-gather of the
+    ``[n_tiles, RT_ZERN_DOUBLES]`` records.  ``backend``: the CPU test seam of ``RayGrid``.
+    ``kwargs``: trace options (``check_apertures``, ...).  Returns a ``ZernikeFit``."""
+    from .parallel import shard_chunks, gather_summaries
+    if not 1 <= num_terms <= E.RT_ZERN_MAX_TERMS:
+        raise ValueError(f'num_terms must be 1 ... {E.RT_ZERN_MAX_TERMS}')
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    fields = list(osp.field_of_view.fields if fields is None else fields)
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    foc = osp.defocus.focus_shift if foc is None else foc
+    tab = None if backend is not None else _table_for(opt_model, table, device)
+    args, grid_kw = wavefront_grid_args(opt_model, tab, num_rays, fields, wvls, foc, image_pt_2d, image_delta,
+                                        backend)
+    ref_img = grid_kw['ref_img']
+    kwargs.setdefault('check_apertures', True)
+    if backend is not None:
+        spec = E.PupilGridSpec(*args, **grid_kw)
+        r = backend.trace_tile(opt_model, spec, True, kwargs['check_apertures'])
+        summ_host = _zernike_sums_host(spec, np.asarray(r['status']), np.asarray(r['opd']), num_terms)
+    else:
+        dev = torch.device('cuda', tab.device)
+        with torch.cuda.device(dev):
+            grid = E.PupilGrid(*args, device=tab.device, **grid_kw)
+            c0, c1 = (0, grid.n_chunks) if shard is None else shard_chunks(grid.n_chunks, *shard)
+            if chunk_range is not None:
+                c0, c1 = chunk_range
+            summ = E.trace_grid_zernike(tab, grid, num_terms, c0, c1, **kwargs)
+            if shard is not None:
+                summ = gather_summaries(summ, group)
+            summ_host = summ.cpu().numpy()                 # one small copy; waits
+            grid.close()
+    lam = np.array([[opt_model.nm_to_sys_units(w) for w in wvls]]*len(fields)).ravel()
+    stats = E.zernike_statistics(summ_host, lam, num_terms)
+    return ZernikeFit(stats, summ_host, ref_img, num_rays, num_terms, len(fields), len(wvls))
+
+
 # --------------------------------------------------------------------------
 # RayFan / RayList / RayGrid: the reference's analysis classes
 # (/root/reference/src/rayoptics/raytr/analyses.py:121-187,343-434,584-663) with

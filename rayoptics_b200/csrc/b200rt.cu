@@ -11,6 +11,8 @@
  *   k_trace_grid[_lean]_wfe     one trace, per-tile sums of the OPD and its least-squares fits
  *   k_reduce_summary            fixed-order per-tile reduction of the chunk sums (_wfe: of the
  *                               wavefront-error sums)
+ *   k_zernike_moments<ROWS>     per-chunk Gram matrix of [OPD, Fringe Zernike terms] from a grid
+ *                               trace's per-ray opd / status; k_reduce_zernike adds the chunks
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
  * The surface table (n_ifc x rt_surface_desc + n_wvl x n_ifc indices) is staged
@@ -31,6 +33,7 @@
 #include "rt_device.cuh"
 #include "rt_lean.cuh"
 #include "rt_grid.cuh"
+#include "rt_zernike.cuh"
 
 using namespace b200rt;
 
@@ -1033,6 +1036,176 @@ __global__ void k_combine_wfe(const double *__restrict__ parts, int n_parts, int
     combine_rows<WfeLayout>(parts, n_parts, n, out);
 }
 
+/* ---- Zernike moments (rt_grid_zernike): per tile the packed Gram matrix of the augmented row
+ * a = [W, Z_1 ... Z_J] of its used rays (status 0, r2 <= 1).  One warp per chunk (256 rays of one
+ * tile).  The warp evaluates a for 32 rays at a time, one ray per lane, into shared memory; then every
+ * lane runs over those 32 rows in ray order and adds a_i*a_j into a fixed register block of ROWS x 8
+ * entries of the triangle.  Every entry is thus one chain over the chunk's rays in ray order, from
+ * +0.0 (DESIGN.md section 4); no atomics.  The chunk's record goes to scratch and k_reduce_zernike
+ * adds the tile's chunk records in chunk order. */
+#define RT_ZERN_WARPS 4          /* warps (= chunks) per CTA of k_zernike_moments */
+#define RT_ZERN_ROW 41           /* shared row stride in doubles: 5 blocks of 8 columns + 1 (odd: stores by
+                                  * 16 lanes to one column hit 16 distinct bank pairs) */
+#define RT_ZERN_HEAD 9           /* record columns before the Gram block */
+
+struct ZernLayout {        /* RT_ZERN_DOUBLES: Zernike moments */
+    static constexpr int W = RT_ZERN_DOUBLES;
+    static __device__ __forceinline__ constexpr bool is_min(int k) { return k == 6; }
+    static __device__ __forceinline__ constexpr bool is_max(int k) { return k == 7; }
+};
+
+/* shared slot of column d of an augmented row: column-major over 5 blocks of 8, so that the 5 block
+ * columns one lane-load instruction touches are adjacent (1 wavefront for the 8-wide block loads, at
+ * most 2 for the row loads) */
+__device__ __forceinline__ int zern_slot(int d) { return (d & 7)*5 + (d >> 3); }
+
+/* ROWS: rows of the lane's register block (4 for J >= 24, 2 for J >= 8, else 1), so that the
+ * triangle's n_blocks (n_blocks + 1)/2 pairs of 8-blocks x 8/ROWS parts fit in 32 lanes */
+template <int ROWS>
+__global__ void __launch_bounds__(RT_ZERN_WARPS*32, 3)
+k_zernike_moments(GridDev G, int64_t chunk_begin, int64_t chunk_end, int n_terms, int n_blocks,
+                  const int32_t *__restrict__ status, const double *__restrict__ opd, double *__restrict__ rec,
+                  int64_t rec_stride)
+{
+    __shared__ double sh[RT_ZERN_WARPS][32*RT_ZERN_ROW];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t c = chunk_begin + (int64_t)blockIdx.x*RT_ZERN_WARPS + warp;
+    if (c >= chunk_end) return;
+    double *A = sh[warp];
+    const int64_t tile = c/G.chunks_per_tile, lc = c - tile*G.chunks_per_tile;
+    const int f = (int)(tile/G.n_wvls);
+    const int64_t tile0 = chunk_begin/G.chunks_per_tile;
+    const int64_t ray0 = tile0*G.rays_per_tile + (chunk_begin - tile0*G.chunks_per_tile)*RT_BLOCK;
+
+    /* the lane's block: pair p of 8-blocks (I <= Jb, numbered Jb-major), rows ROWS*part ... of block I */
+    constexpr int PARTS = 8/ROWS;
+    const int p = lane/PARTS, part = lane - p*PARTS;
+    int I = p, Jb = 0;
+    while (Jb < 5 && I > Jb) { I -= Jb + 1; Jb++; }
+    const bool active = Jb < n_blocks;
+    if (!active) { I = 0; Jb = 0; }               /* computes a block it does not store */
+    const int i0 = 8*I + ROWS*part, j0 = 8*Jb;
+    int si[ROWS], sj[8];
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) si[k] = zern_slot(i0 + k);
+#pragma unroll
+    for (int q = 0; q < 8; q++) sj[q] = zern_slot(j0 + q);
+
+    double acc[ROWS][8];
+#pragma unroll
+    for (int k = 0; k < ROWS; k++)
+#pragma unroll
+        for (int q = 0; q < 8; q++) acc[k][q] = 0.0;
+    int cnt[5] = {0, 0, 0, 0, 0}, n_used = 0;     /* lane 0's */
+    double mn = CUDART_INF, mx = -CUDART_INF;
+    const int n_cols = 8*n_blocks;
+    double *row = A + lane*RT_ZERN_ROW;
+    for (int s = 0; s < RT_WARPS; s++) {
+        const int64_t loc = lc*RT_BLOCK + s*32 + lane;
+        const bool have = loc < G.rays_per_tile;
+        int st = 0;
+        double W = 0.0, x = 0.0, y = 0.0;
+        if (have) {
+            const int64_t k = tile*G.rays_per_tile + loc - ray0;
+            st = status[k];
+            W = opd[k];
+            grid_pupil_coords(G, f, loc, x, y);
+        }
+        const bool used = have && st == RT_RAY_OK && x*x + y*y <= 1.0;
+        const int ck = (st >= 0 && st <= RT_RAY_BLOCKED) ? st : 4;
+#pragma unroll
+        for (int cl = 0; cl < 5; cl++) cnt[cl] += __popc(__ballot_sync(0xffffffffu, have && ck == cl));
+        n_used += __popc(__ballot_sync(0xffffffffu, used));
+        if (used) { mn = fmin(mn, W); mx = fmax(mx, W); }
+        /* the augmented row of this lane's ray; +0.0 for a ray that is not used and past J */
+        row[zern_slot(0)] = used ? W : 0.0;
+        fringe_zernike(x, y, n_terms, [&](int j, double z) { row[zern_slot(j)] = used ? z : 0.0; });
+        for (int d = n_terms + 1; d < n_cols; d++) row[zern_slot(d)] = 0.0;
+        __syncwarp();
+#pragma unroll 4
+        for (int r = 0; r < 32; r++) {
+            const double *ar = A + r*RT_ZERN_ROW;
+            double ai[ROWS], aj[8];
+#pragma unroll
+            for (int k = 0; k < ROWS; k++) ai[k] = ar[si[k]];
+#pragma unroll
+            for (int q = 0; q < 8; q++) aj[q] = ar[sj[q]];
+#pragma unroll
+            for (int k = 0; k < ROWS; k++)
+#pragma unroll
+                for (int q = 0; q < 8; q++) acc[k][q] = acc[k][q] + ai[k]*aj[q];
+        }
+        __syncwarp();
+    }
+    double *out = rec + (c - chunk_begin)*rec_stride;
+    if (active) {
+#pragma unroll
+        for (int k = 0; k < ROWS; k++)
+#pragma unroll
+            for (int q = 0; q < 8; q++) {
+                const int i = i0 + k, j = j0 + q;
+                if (i <= j && j <= n_terms) out[RT_ZERN_HEAD + j*(j + 1)/2 + i] = acc[k][q];
+            }
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        mn = fmin(mn, __shfl_xor_sync(0xffffffffu, mn, off));
+        mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int cl = 0; cl < 5; cl++) out[cl] = (double)cnt[cl];
+        out[5] = (double)n_used;
+        out[6] = mn;
+        out[7] = mx;
+        out[8] = 0.0;
+    }
+}
+
+/* one thread per (tile, record column): the tile's chunk records inside the range added in chunk
+ * order from +0.0 (counts too; column 6 fmin, 7 fmax).  Columns past the launch's record width and
+ * tiles without chunks in the range get the identity.  The chain is sequential, so the loads of
+ * RT_ZERN_RED_BATCH chunks are issued before their additions: one memory latency per batch. */
+#define RT_ZERN_RED_THREADS 64
+#define RT_ZERN_RED_BATCH 32
+__global__ void __launch_bounds__(RT_ZERN_RED_THREADS)
+k_reduce_zernike(const double *__restrict__ rec, int64_t rec_stride, int64_t chunk_begin, int64_t chunk_end,
+                 int64_t chunks_per_tile, int64_t n_tiles, double *__restrict__ summary)
+{
+    const int64_t i = (int64_t)blockIdx.x*blockDim.x + threadIdx.x;
+    if (i >= n_tiles*RT_ZERN_DOUBLES) return;
+    const int64_t tile = i/RT_ZERN_DOUBLES;
+    const int k = (int)(i - tile*RT_ZERN_DOUBLES);
+    double v = red_identity<ZernLayout>(k);
+    if (k < rec_stride) {
+        const int64_t c0 = tile*chunks_per_tile > chunk_begin ? tile*chunks_per_tile : chunk_begin;
+        const int64_t c1 = (tile + 1)*chunks_per_tile < chunk_end ? (tile + 1)*chunks_per_tile : chunk_end;
+        const double *p = rec + (c0 - chunk_begin)*rec_stride + k;
+        int64_t c = c0;
+        for (; c + RT_ZERN_RED_BATCH <= c1; c += RT_ZERN_RED_BATCH, p += RT_ZERN_RED_BATCH*rec_stride) {
+            double b[RT_ZERN_RED_BATCH];
+#pragma unroll
+            for (int q = 0; q < RT_ZERN_RED_BATCH; q++) b[q] = p[q*rec_stride];
+#pragma unroll
+            for (int q = 0; q < RT_ZERN_RED_BATCH; q++) v = red_op<ZernLayout>(k, v, b[q]);
+        }
+        for (; c < c1; c++, p += rec_stride) v = red_op<ZernLayout>(k, v, *p);
+    }
+    summary[i] = v;
+}
+
+__global__ void k_zernike_identity(double *__restrict__ summary, int64_t n)
+{
+    const int64_t i = (int64_t)blockIdx.x*blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    summary[i] = red_identity<ZernLayout>((int)(i % RT_ZERN_DOUBLES));
+}
+
+__global__ void k_combine_zernike(const double *__restrict__ parts, int n_parts, int64_t n, double *__restrict__ out)
+{
+    combine_rows<ZernLayout>(parts, n_parts, n, out);
+}
+
 /* chief rays of all fields: pupil (0, 0), no vignetting, apertures not checked, general
  * per-ray code on the global table (bit-identical to the lean loop by construction, and
  * n_fields rays do not need the specialised kernel).  One thread per field. */
@@ -1958,6 +2131,69 @@ int rt_combine_wfe(const double *parts, int32_t n_parts, int64_t n_tiles, double
     if (n_tiles == 0) return RT_OK;
     const int64_t n = n_tiles*RT_WFE_DOUBLES;
     k_combine_wfe<<<(unsigned)((n + 255)/256), 256, 0, (cudaStream_t)stream>>>(parts, n_parts, n, out);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+/* doubles of one chunk record of rt_grid_zernike: the head and the packed Gram block of J terms */
+static int64_t zern_rec_stride(int32_t n_terms)
+{
+    return RT_ZERN_HEAD + (int64_t)(n_terms + 1)*(n_terms + 2)/2;
+}
+
+int64_t rt_grid_zernike_scratch_bytes(const rt_grid *g, int64_t chunk_begin, int64_t chunk_end, int32_t n_terms)
+{
+    if (!g || chunk_begin < 0 || chunk_end < chunk_begin || chunk_end > g->n_chunks || n_terms < 1 ||
+        n_terms > RT_ZERN_MAX_TERMS)
+        return 0;
+    return (chunk_end - chunk_begin)*zern_rec_stride(n_terms)*(int64_t)sizeof(double);
+}
+
+int rt_grid_zernike(const rt_grid *g, int64_t chunk_begin, int64_t chunk_end, int32_t n_terms,
+                    const int32_t *status, const double *opd, double *summary, void *scratch, void *stream)
+{
+    if (!g || !summary) return fail(RT_ERR_INVALID, "rt_grid_zernike: grid and summary are required");
+    if (n_terms < 1 || n_terms > RT_ZERN_MAX_TERMS) return fail(RT_ERR_INVALID, "rt_grid_zernike: n_terms must be 1 ... 37");
+    if (chunk_begin < 0 || chunk_end > g->n_chunks || chunk_end < chunk_begin)
+        return fail(RT_ERR_INVALID, "rt_grid_zernike: chunk range out of bounds");
+    if (g->paired) return fail(RT_ERR_INVALID, "rt_grid_zernike: needs a product grid (paired = 0)");
+    if (g->apply_vignetting)
+        return fail(RT_ERR_INVALID, "rt_grid_zernike: the pupil coordinates must not be vignetted (apply_vignetting = 0)");
+    if (chunk_end > chunk_begin && (!status || !opd || !scratch))
+        return fail(RT_ERR_INVALID, "rt_grid_zernike: status, opd and scratch are required");
+    DeviceGuard guard(g->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (chunk_begin == chunk_end) {
+        const int64_t n = g->n_tiles*RT_ZERN_DOUBLES;
+        k_zernike_identity<<<(unsigned)((n + 255)/256), 256, 0, s>>>(summary, n);
+        g_launches++;
+        CUDA_TRY(cudaGetLastError());
+        return RT_OK;
+    }
+    const int64_t stride = zern_rec_stride(n_terms);
+    const int n_blocks = (n_terms + 1 + 7)/8, pairs = n_blocks*(n_blocks + 1)/2;
+    const GridDev G = grid_dev(g);
+    double *rec = (double *)scratch;
+    const unsigned blocks = (unsigned)((chunk_end - chunk_begin + RT_ZERN_WARPS - 1)/RT_ZERN_WARPS);
+    auto kern = pairs*8 <= 32 ? k_zernike_moments<1> : (pairs*4 <= 32 ? k_zernike_moments<2> : k_zernike_moments<4>);
+    kern<<<blocks, RT_ZERN_WARPS*32, 0, s>>>(G, chunk_begin, chunk_end, n_terms, n_blocks, status, opd, rec, stride);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    const int64_t n = g->n_tiles*RT_ZERN_DOUBLES;
+    k_reduce_zernike<<<(unsigned)((n + RT_ZERN_RED_THREADS - 1)/RT_ZERN_RED_THREADS), RT_ZERN_RED_THREADS, 0, s>>>(
+        rec, stride, chunk_begin, chunk_end, g->chunks_per_tile, g->n_tiles, summary);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+int rt_combine_zernike(const double *parts, int32_t n_parts, int64_t n_tiles, double *out, void *stream)
+{
+    if (!parts || !out || n_parts < 1 || n_tiles < 0) return fail(RT_ERR_INVALID, "rt_combine_zernike: bad arguments");
+    if (n_tiles == 0) return RT_OK;
+    const int64_t n = n_tiles*RT_ZERN_DOUBLES;
+    k_combine_zernike<<<(unsigned)((n + 255)/256), 256, 0, (cudaStream_t)stream>>>(parts, n_parts, n, out);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RT_OK;

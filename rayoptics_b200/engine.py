@@ -19,7 +19,8 @@ import numpy as np
 import torch
 
 from . import _abi
-from ._abi import rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES, RT_WFE_DOUBLES
+from ._abi import (rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES, RT_WFE_DOUBLES,
+                   RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS)
 
 SUMMARY_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other',
                   'sum_x', 'sum_y', 'sum_xx', 'sum_yy', 'sum_xy',
@@ -31,7 +32,10 @@ WFE_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other', 'min_w', 'max
               'sum_x', 'sum_y', 'sum_xx', 'sum_xy', 'sum_yy', 'sum_xr2', 'sum_yr2', 'sum_r2r2',
               'reserved0', 'reserved1', 'reserved2', 'reserved3')
 # min / max columns of the two record layouts, by record width
-_MINMAX_COLS = {RT_SUMMARY_DOUBLES: ((10, 12), (11, 13)), RT_WFE_DOUBLES: ((5,), (6,))}
+_MINMAX_COLS = {RT_SUMMARY_DOUBLES: ((10, 12), (11, 13)), RT_WFE_DOUBLES: ((5,), (6,)),
+                RT_ZERN_DOUBLES: ((6,), (7,))}
+_COMBINE_FN = {RT_SUMMARY_DOUBLES: 'rt_combine_summaries', RT_WFE_DOUBLES: 'rt_combine_wfe',
+               RT_ZERN_DOUBLES: 'rt_combine_zernike'}
 
 
 def _ptr(t):
@@ -495,11 +499,11 @@ def decode_nan_status(abr):
 
 
 def combine_summaries(parts, out=None):
-    """Combine partial ``[n_tiles, 16]`` spot summaries or ``[n_tiles, RT_WFE_DOUBLES]``
-    wavefront-error records (from chunk ranges / ranks; the layout is chosen by ``shape[-1]``):
-    sums add in part order, min/max columns take min/max.  CUDA tensors: one
-    ``rt_combine_summaries`` / ``rt_combine_wfe`` launch on the current stream; CPU tensors (gloo
-    tests): torch."""
+    """Combine partial ``[n_tiles, 16]`` spot summaries, ``[n_tiles, RT_WFE_DOUBLES]``
+    wavefront-error records or ``[n_tiles, RT_ZERN_DOUBLES]`` Zernike moments records (from chunk
+    ranges / ranks; the layout is chosen by ``shape[-1]``): sums add in part order, min/max columns
+    take min/max.  CUDA tensors: one ``rt_combine_summaries`` / ``rt_combine_wfe`` /
+    ``rt_combine_zernike`` launch on the current stream; CPU tensors (gloo tests): torch."""
     parts = torch.stack(list(parts)) if not torch.is_tensor(parts) else parts
     width = parts.shape[-1]
     if width not in _MINMAX_COLS:
@@ -509,7 +513,7 @@ def combine_summaries(parts, out=None):
         if out is None:
             out = torch.empty(parts.shape[1:], dtype=parts.dtype, device=parts.device)
         lib = _abi.load_library()
-        fn = lib.rt_combine_summaries if width == RT_SUMMARY_DOUBLES else lib.rt_combine_wfe
+        fn = getattr(lib, _COMBINE_FN[width])
         with torch.cuda.device(parts.device):
             _abi.check(fn(_ptr(parts), parts.shape[0], parts.shape[1], _ptr(out), _stream_ptr(parts.device)))
         out._keep = parts
@@ -631,6 +635,143 @@ def wavefront_statistics(summary, wvl_sys):
         c4, rss4 = _fit(g4, np.array([sw, sxw, syw, sr2w]), sww, nt)
         out['rms_focus'][t] = np.sqrt(max(rss4, 0.0)/nt)/lt if np.isfinite(rss4) else np.nan
         out['focus'][t] = c4[3]/lt
+    if is_t:
+        return {k: torch.as_tensor(v, device=summary.device) for k, v in out.items()}
+    return out
+
+
+# --- Fringe Zernike fits (rt_grid_zernike; the polynomials of csrc/rt_zernike.cuh) --------------
+# (n, m, 'cos' | 'sin' | None, integer coefficients of P from the constant term up), Fringe order:
+# Z_j = R_n^m(rho) * cos | sin(m theta), R_n^m(rho) = rho^m * P(rho^2), theta from +x
+FRINGE_TERMS = (
+    (0, 0, None, (1,)), (1, 1, 'cos', (1,)), (1, 1, 'sin', (1,)), (2, 0, None, (-1, 2)),
+    (2, 2, 'cos', (1,)), (2, 2, 'sin', (1,)), (3, 1, 'cos', (-2, 3)), (3, 1, 'sin', (-2, 3)),
+    (4, 0, None, (1, -6, 6)), (3, 3, 'cos', (1,)), (3, 3, 'sin', (1,)), (4, 2, 'cos', (-3, 4)),
+    (4, 2, 'sin', (-3, 4)), (5, 1, 'cos', (3, -12, 10)), (5, 1, 'sin', (3, -12, 10)),
+    (6, 0, None, (-1, 12, -30, 20)), (4, 4, 'cos', (1,)), (4, 4, 'sin', (1,)), (5, 3, 'cos', (-4, 5)),
+    (5, 3, 'sin', (-4, 5)), (6, 2, 'cos', (6, -20, 15)), (6, 2, 'sin', (6, -20, 15)),
+    (7, 1, 'cos', (-4, 30, -60, 35)), (7, 1, 'sin', (-4, 30, -60, 35)), (8, 0, None, (1, -20, 90, -140, 70)),
+    (5, 5, 'cos', (1,)), (5, 5, 'sin', (1,)), (6, 4, 'cos', (-5, 6)), (6, 4, 'sin', (-5, 6)),
+    (7, 3, 'cos', (10, -30, 21)), (7, 3, 'sin', (10, -30, 21)), (8, 2, 'cos', (-10, 60, -105, 56)),
+    (8, 2, 'sin', (-10, 60, -105, 56)), (9, 1, 'cos', (5, -60, 210, -280, 126)),
+    (9, 1, 'sin', (5, -60, 210, -280, 126)), (10, 0, None, (-1, 30, -210, 560, -630, 252)),
+    (12, 0, None, (1, -42, 420, -1680, 3150, -2772, 924)))
+ZERN_HEAD = 9            # record columns before the packed Gram block (include/b200rt.h)
+
+
+def zernike_terms(x, y, n_terms=RT_ZERN_MAX_TERMS):
+    """``[..., n_terms]`` Fringe Zernike terms Z_1 ... Z_n_terms at relative pupil coordinates
+    ``(x, y)``, bit for bit as the device evaluates them (csrc/rt_zernike.cuh): r2 = x*x + y*y;
+    C1 = x, S1 = y, C(k+1) = C(k)*x - S(k)*y, S(k+1) = S(k)*x + C(k)*y; P by Horner in r2 from the
+    highest coefficient; Z = P*C(m), P*S(m) or P.  Every product is rounded once."""
+    if not 1 <= n_terms <= RT_ZERN_MAX_TERMS:
+        raise ValueError(f'n_terms must be 1 ... {RT_ZERN_MAX_TERMS}')
+    x, y = np.broadcast_arrays(np.asarray(x, dtype=np.float64), np.asarray(y, dtype=np.float64))
+    with np.errstate(all='ignore'):
+        r2 = x*x + y*y
+        C, S = [None, x], [None, y]
+        for k in range(1, 5):
+            C.append(C[k]*x - S[k]*y)
+            S.append(S[k]*x + C[k]*y)
+        out = np.empty(x.shape + (n_terms,))
+        for j, (n, m, kind, a) in enumerate(FRINGE_TERMS[:n_terms]):
+            p = np.full(x.shape, float(a[-1]))
+            for c in a[-2::-1]:
+                p = p*r2 + float(c)
+            out[..., j] = p if m == 0 else p*(S[m] if kind == 'sin' else C[m])
+    return out
+
+
+def zernike_gram_col(i, j):
+    """record column of the Gram entry sum a_i*a_j (a_0 = W, a_k = Z_k; symmetric in i, j)"""
+    i, j = min(i, j), max(i, j)
+    return ZERN_HEAD + j*(j + 1)//2 + i
+
+
+def zernike_gram(record, n_terms):
+    """``[..., n_terms + 1, n_terms + 1]`` symmetric Gram matrices of [W, Z_1 ... Z_n_terms] from
+    ``[..., RT_ZERN_DOUBLES]`` records"""
+    s = np.asarray(record, dtype=np.float64)
+    idx = np.array([[zernike_gram_col(i, j) for j in range(n_terms + 1)] for i in range(n_terms + 1)])
+    return s[..., idx]
+
+
+def grid_zernike(grid, chunk_begin, chunk_end, n_terms, status, opd):
+    """``rt_grid_zernike``: the ``[n_tiles, RT_ZERN_DOUBLES]`` Zernike moments record (float64
+    device tensor) of chunks ``[chunk_begin, chunk_end)`` of a product PupilGrid without vignetting,
+    from the per-ray ``status`` (int32) and ``opd`` (float64, system units) device tensors of a grid
+    trace over the same chunks.  Asynchronous on the current CUDA stream."""
+    lib = _abi.load_library()
+    n = grid.rays_in_chunks(chunk_begin, chunk_end)
+    for t, dt, name in ((status, torch.int32, 'status'), (opd, torch.float64, 'opd')):
+        if not (torch.is_tensor(t) and t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n):
+            raise ValueError(f'{name} must be a contiguous {dt} CUDA tensor of the {n} rays of the chunk range')
+    device = status.device
+    summ = torch.empty((grid.n_tiles, RT_ZERN_DOUBLES), dtype=torch.float64, device=device)
+    nbytes = lib.rt_grid_zernike_scratch_bytes(grid.handle, chunk_begin, chunk_end, n_terms)
+    scratch = torch.empty(max(nbytes//8, 1), dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        _abi.check(lib.rt_grid_zernike(grid.handle, chunk_begin, chunk_end, n_terms, _ptr(status), _ptr(opd),
+                                       _ptr(summ), _ptr(scratch), _stream_ptr(device)))
+    summ._keep = (scratch, status, opd)        # must outlive the asynchronous launches
+    return summ
+
+
+def trace_grid_zernike(table, grid, n_terms, chunk_begin=0, chunk_end=None, res=None, **kwargs):
+    """Zernike moments of chunks ``[chunk_begin, chunk_end)`` of a PupilGrid built with ``wave=``
+    records: ``trace_grid`` with the ``opd`` and ``status`` outputs into device buffers (``res``:
+    an optional BundleResult with both, which keeps them), then ``grid_zernike``.  Returns the
+    ``[n_tiles, RT_ZERN_DOUBLES]`` device tensor.  Trace defaults as ``trace_grid``."""
+    if chunk_end is None:
+        chunk_end = grid.n_chunks
+    n = grid.rays_in_chunks(chunk_begin, chunk_end)
+    if res is None:
+        res = BundleResult(n, table.n_ifc, torch.device('cuda', table.device), ('opd', 'status'))
+    elif res.opd is None or res.status is None:
+        raise ValueError('res needs the opd and status outputs')
+    trace_grid(table, grid, chunk_begin, chunk_end, summary=False, res=res, **kwargs)
+    summ = grid_zernike(grid, chunk_begin, chunk_end, n_terms, res.status, res.opd)
+    summ._keep = (summ._keep, res)
+    return summ
+
+
+ZERN_STATISTICS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other', 'n_used', 'rms', 'pv', 'rms_residual')
+
+
+def zernike_statistics(summary, wvl_sys, n_terms):
+    """Per-tile Fringe Zernike fit from combined ``[n_tiles, RT_ZERN_DOUBLES]`` records (numpy
+    array or torch tensor; same type out, on the same device).  ``wvl_sys``: the wavelength in
+    system units, a scalar or one value per tile; results in waves.
+
+    ``coef`` ``[n_tiles, n_terms]``: least-squares coefficients of W on Z_1 ... Z_n_terms over the
+    used rays (``_fit`` on the normal equations); ``rms_residual``: sqrt(RSS/n_used); ``rms``:
+    sqrt(sum W^2/n - (sum W/n)^2), piston removed; ``pv``: max W - min W; the counts.  A fit with
+    fewer used rays than terms or a rank-deficient scaled Gram matrix is NaN; a tile without a used
+    ray is NaN everywhere except the counts."""
+    if not 1 <= n_terms <= RT_ZERN_MAX_TERMS:
+        raise ValueError(f'n_terms must be 1 ... {RT_ZERN_MAX_TERMS}')
+    is_t = torch.is_tensor(summary)
+    s = (summary.detach().cpu().numpy() if is_t else np.asarray(summary, dtype=np.float64)).reshape(-1, RT_ZERN_DOUBLES)
+    nt = s.shape[0]
+    lam = np.broadcast_to(np.asarray(wvl_sys, dtype=np.float64).reshape(-1), (nt,))
+    out = {k: s[:, i].copy() for i, k in enumerate(ZERN_STATISTICS[:6])}
+    for k in ZERN_STATISTICS[6:]:
+        out[k] = np.full(nt, np.nan)
+    out['coef'] = np.full((nt, n_terms), np.nan)
+    gram = zernike_gram(s, n_terms)
+    for t in range(nt):
+        n = s[t, 5]
+        if not n > 0:
+            continue
+        g, lt = gram[t], lam[t]
+        sww = g[0, 0]
+        with np.errstate(invalid='ignore'):
+            mean = g[0, 1]/n
+            out['rms'][t] = np.sqrt(max(sww/n - mean*mean, 0.0))/lt if np.isfinite(sww) else np.nan
+        out['pv'][t] = (s[t, 7] - s[t, 6])/lt
+        c, rss = _fit(g[1:, 1:], g[0, 1:], sww, n)
+        out['coef'][t] = c/lt
+        out['rms_residual'][t] = np.sqrt(max(rss, 0.0)/n)/lt if np.isfinite(rss) else np.nan
     if is_t:
         return {k: torch.as_tensor(v, device=summary.device) for k, v in out.items()}
     return out
