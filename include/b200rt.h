@@ -421,6 +421,35 @@ int rt_grid_zernike(const rt_grid *grid, int64_t chunk_begin, int64_t chunk_end,
  * column 7 fmax.  One launch on `stream`. */
 int rt_combine_zernike(const double *parts, int32_t n_parts, int64_t n_tiles, double *out, void *stream);
 
+/* ---- chief-ray aiming (ABI 6, additive): the aim point of every field of a grid, found on the
+ * device by the damped 2-D Newton iteration of vigcalc.aim_chief_ray / aim_all_fields_batched
+ * (csrc/rt_aim.cuh; DESIGN.md section 4).  Per field, starting from aim (0, 0): the (0, 0) pupil ray
+ * of the 'epd' start-ray rule (rt_field_desc pt0, the grid's eprad, z_pupil and flip_z_dir) with the
+ * trial aim in place of rt_field_desc.aim is traced at row wvl_idx of the table with the general
+ * loop (first_surf 1, apertures not checked, intersect_obj on) up to interface `stop`; the iteration
+ * drives its (x, y) intercept there to 0.  h: the forward-difference step, 1e-4*max(1, enp_radius)
+ * in aim_chief_ray; tol: max|intercept| below which a field has converged; max_iter: Newton steps.
+ * aim_out: DEVICE [n_fields][2] receives the aim points (x = 0 is NOT forced for fields with
+ * x = 0: aim_chief_ray applies that rule after its iteration, the caller does it after the copy);
+ * term_out: DEVICE [n_fields] or NULL receives each field's rt_aim_term.  The grid's field records
+ * are read, not changed.  One launch on `stream`, one thread per field.
+ * RT_ERR_UNSUPPORTED before any device work when the grid's pupil_kind is not RT_PUPIL_EPD
+ * (wide-angle fields and angular pupils stay with the host functions); RT_ERR_INVALID before any
+ * device work when stop is not in 1 ... n_ifc - 2, wvl_idx is out of range, h or tol is not finite
+ * and positive, max_iter < 0 or aim_out is NULL. */
+enum rt_aim_term {
+    RT_AIM_CONVERGED = 0,    /* max|intercept| < tol */
+    RT_AIM_FIRST_FAILED = 1, /* the ray aimed at (0, 0) does not reach the stop: aim (0, 0) */
+    RT_AIM_DIFF_FAILED = 2,  /* a forward-difference ray does not reach the stop */
+    RT_AIM_SINGULAR = 3,     /* zero pivot in the 2x2 solve, or a step that is not finite */
+    RT_AIM_NO_STEP = 4,      /* none of the 20 backtracking trials reduced max|intercept| (the usual
+                                end for objects at infinity: the noise floor of the intercept) */
+    RT_AIM_MAX_ITER = 5      /* max_iter Newton steps taken */
+};
+int rt_grid_aim_chief(const rt_table *table, const rt_grid *grid, int32_t stop, int32_t wvl_idx,
+                      double h, double tol, int32_t max_iter, double *aim_out, int32_t *term_out,
+                      void *stream);
+
 /* ---- misc */
 const char *rt_last_error(void);
 int rt_abi_version(void);

@@ -31,6 +31,8 @@ PUPIL_EPD, PUPIL_NA, PUPIL_FNO, PUPIL_WIDE = 0, 1, 2, 3
 MODE_IDS = {'transmit': 0, 'reflect': 1, 'dummy': 2, 'phantom': 3}
 # enum rt_status
 RAY_OK, RAY_MISSED, RAY_TIR, RAY_BLOCKED, RAY_EVANESCENT, RAY_NUMERIC = range(6)
+# enum rt_aim_term
+AIM_CONVERGED, AIM_FIRST_FAILED, AIM_DIFF_FAILED, AIM_SINGULAR, AIM_NO_STEP, AIM_MAX_ITER = range(6)
 # enum rt_aperture_type
 APERTURE_IDS = {'Circular': 1, 'Rectangular': 2, 'Elliptical': 3}
 
@@ -122,7 +124,7 @@ EXPORTS = ['rt_table_create', 'rt_table_destroy', 'rt_table_dims', 'rt_table_set
            'rt_last_error', 'rt_abi_version', 'rt_chunk_rays', 'rt_launch_count', 'rt_measure_fp64_peak', 'rt_measure_fp64_latency',
            'rt_selftest_division', 'rt_grid_chief_ref_focus', 'rt_grid_focus_scratch_bytes',
            'rt_trace_grid_focus', 'rt_grid_wfe_scratch_bytes', 'rt_trace_grid_wfe', 'rt_combine_wfe',
-           'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike']
+           'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike', 'rt_grid_aim_chief']
 
 _lib = None
 
@@ -196,6 +198,8 @@ def load_library():
     lib.rt_grid_zernike.restype = i32
     lib.rt_combine_zernike.argtypes = [vp, i32, i64, vp, vp]
     lib.rt_combine_zernike.restype = i32
+    lib.rt_grid_aim_chief.argtypes = [vp, vp, i32, i32, C.c_double, C.c_double, i32, vp, vp, vp]
+    lib.rt_grid_aim_chief.restype = i32
     lib.rt_last_error.restype = C.c_char_p
     lib.rt_abi_version.restype = i32
     lib.rt_chunk_rays.restype = i32

@@ -24,6 +24,7 @@ import torch
 
 from . import engine as E
 from .table import SurfaceTable
+from .model import Field
 from .opticalspec import grid_fields_of
 
 
@@ -512,6 +513,126 @@ def zernike_fit(opt_model, num_rays=64, num_terms=37, fields=None, wvls=None, fo
     lam = np.array([[opt_model.nm_to_sys_units(w) for w in wvls]]*len(fields)).ravel()
     stats = E.zernike_statistics(summ_host, lam, num_terms)
     return ZernikeFit(stats, summ_host, ref_img, num_rays, num_terms, len(fields), len(wvls))
+
+
+class FieldMap:
+    """Result of ``field_map``: a ``num_fields`` x ``num_fields`` grid of field points over the
+    relative field [-1, 1]^2 (x outer, y inner).
+
+    ``field_x``, ``field_y`` ``[n, n]``: the points' Field.x / Field.y (field-of-view units);
+    ``traced`` ``[n, n]``: the point lies inside the unit circle of relative field and was aimed;
+    ``valid`` ``[n, n]``: it was aimed and its chief ray reaches the image at every wavelength (the
+    points with results); ``aim`` ``[n, n, 2]``: the aim points; ``img`` ``[n, n, n_wvls, 2]``: the
+    real chief-ray image points (``ZernikeFit.ref_img``); ``parax_img`` ``[n, n, 2]``: the paraxial
+    image points; ``distortion`` ``[n, n, n_wvls]`` in percent; ``coef`` ``[n, n, n_wvls,
+    num_terms]`` Fringe Zernike coefficients, ``rms``, ``rms_residual``, ``pv`` ``[n, n, n_wvls]``, in
+    waves; ``zernike``: the ``ZernikeFit`` of the valid points in row-major order of the map; ``wvls``.
+    Entries without a result are NaN."""
+
+    def __init__(self, **kw):
+        for k, v in kw.items():
+            setattr(self, k, v)
+
+
+def paraxial_image_points(opt_model, fx, fy):
+    """Paraxial image points ``[..., 2]`` of the fields (fx, fy) (field-of-view units): the chief
+    ray's paraxial image height ``pr_ray[-1][HT]`` scaled linearly with the field variable the
+    paraxial model is built on -- for object angles the slopes (d_x/d_z, d_y/d_z) of the object-space
+    direction ``obj_coords`` gives the field, (tan a_x, tan a_y/cos a_x), against ``fod.pr_slp0``
+    (tan(angle) on the x and y axes of the field); for object heights the height against
+    ``fod.pr_ht0``.  NaN for every other field specification and for wide-angle fields."""
+    from .firstorder import HT
+    osp = opt_model.optical_spec
+    fov, fod = osp.field_of_view, osp.fod
+    fx, fy = np.asarray(fx, dtype=np.float64), np.asarray(fy, dtype=np.float64)
+    scale = fov.value if fov.is_relative else 1.0
+    key = tuple(fov.key)
+    if fov.is_wide_angle or key not in (('object', 'angle'), ('object', 'height')):
+        return np.full(fx.shape + (2,), np.nan)
+    if key == ('object', 'angle'):
+        ax, ay = np.deg2rad(scale*fx), np.deg2rad(scale*fy)
+        dz = np.cos(ax)*np.cos(ay)
+        ux, uy = np.sin(ax)*np.cos(ay)/dz, np.sin(ay)/dz
+        umax = fod.pr_slp0
+    else:
+        ux, uy = scale*fx, scale*fy
+        umax = fod.pr_ht0
+    h = fod.pr_ray[-1][HT]
+    return np.stack([h*ux/umax, h*uy/umax], axis=-1)
+
+
+def field_map(opt_model, num_fields=9, num_rays=32, num_terms=37, wvls=None, foc=None, table=None, device=0,
+              backend=None, **trace_kwargs):
+    """Full-field maps of the wavefront (Fringe Zernike fit, RMS, P-V) and of distortion over a
+    ``num_fields`` x ``num_fields`` grid of field points.
+
+    The points are ``np.linspace(-1, 1, num_fields)`` in x (outer) and y (inner) of relative field,
+    each a ``Field`` scaled by ``fov.max_field()[0]`` with zero vignetting factors; points with
+    sqrt(x^2 + y^2) > 1 are not traced.  Steps: (1) the chief rays of all points are aimed on the
+    device at the central wavelength (``vigcalc.aim_fields_on_device``: one launch); (2) one chief-ray
+    launch (``waveabr.trace_chief_rays``) drops the points whose chief ray misses the image at any
+    wavelength; (3) one ``zernike_fit`` over the remaining points.
+
+    Distortion = 100 (|p_real| - |p_par|)/|p_par| with p_real the real chief ray's image point and
+    p_par = ``paraxial_image_points`` (linear in the object-space chief-ray slope or object height): defined for object-angle and object-height fields that are not
+    wide-angle, NaN for every other field specification (image heights included) and on the axis.
+    ``backend``: the CPU test seam -- ``backend.aim_fields(opt_model, fields, wvl)`` aims like
+    ``aim_fields_on_device``, ``backend.chief_rays`` / ``trace_tile`` as ``zernike_fit``'s.
+    ``trace_kwargs``: trace options of ``zernike_fit``.  Returns a ``FieldMap``."""
+    from . import vigcalc as V
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    fov = osp.field_of_view
+    n = int(num_fields)
+    if n < 1:
+        raise ValueError('num_fields must be at least 1')
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    nw = len(wvls)
+    rel = np.linspace(-1.0, 1.0, n)
+    rx, ry = np.meshgrid(rel, rel, indexing='ij')
+    scale = fov.max_field()[0]
+    if fov.is_relative and fov.value != 0:
+        scale = scale/fov.value
+    field_x, field_y = scale*rx, scale*ry
+    traced = np.sqrt(rx*rx + ry*ry) <= 1.0
+    pts = [(i, j) for i in range(n) for j in range(n) if traced[i, j]]
+    fields = [Field(x=float(field_x[i, j]), y=float(field_y[i, j]), fov=fov) for i, j in pts]
+    tab = None if backend is not None else _table_for(opt_model, table, device)
+    cwl = osp.spectral_region.central_wvl
+    if backend is not None:
+        backend.aim_fields(opt_model, fields, cwl)
+    else:
+        V.aim_fields_on_device(opt_model, fields, cwl, table=tab, device=device)
+    if fields:
+        _, _, status = (W.trace_chief_rays(opt_model, tab, fields, wvls) if backend is None
+                        else backend.chief_rays(opt_model, fields, wvls))
+        ok = (np.asarray(status).reshape(len(fields), nw) == 0).all(axis=1)
+    else:
+        ok = np.zeros(0, dtype=bool)
+    kept = [fld for fld, k in zip(fields, ok) if k]
+    where = [p for p, k in zip(pts, ok) if k]
+    zf = None
+    if kept:
+        zf = zernike_fit(opt_model, num_rays, num_terms, fields=kept, wvls=wvls, foc=foc, table=table,
+                         device=device, backend=backend, **trace_kwargs)
+    nan = lambda *shape: np.full(shape, np.nan)        # noqa: E731
+    aim, img, coef = nan(n, n, 2), nan(n, n, nw, 2), nan(n, n, nw, num_terms)
+    rms, rms_res, pv = nan(n, n, nw), nan(n, n, nw), nan(n, n, nw)
+    valid = np.zeros((n, n), dtype=bool)
+    for (i, j), fld in zip(pts, fields):
+        aim[i, j] = fld.aim_info
+    for k, (i, j) in enumerate(where):
+        valid[i, j] = True
+        img[i, j], coef[i, j] = zf.ref_img[k], zf.coef[k]
+        rms[i, j], rms_res[i, j], pv[i, j] = zf.rms[k], zf.rms_residual[k], zf.pv[k]
+    parax = paraxial_image_points(opt_model, field_x, field_y)
+    parax[~traced] = np.nan
+    r_par = np.hypot(parax[..., 0], parax[..., 1])[..., None]
+    r_real = np.hypot(img[..., 0], img[..., 1])
+    with np.errstate(invalid='ignore', divide='ignore'):
+        dist = np.where(r_par > 0, 100.0*(r_real - r_par)/r_par, np.nan)
+    return FieldMap(field_x=field_x, field_y=field_y, traced=traced, valid=valid, aim=aim, img=img,
+                    parax_img=parax, distortion=dist, coef=coef, rms=rms, rms_residual=rms_res, pv=pv,
+                    zernike=zf, wvls=wvls, num_rays=num_rays, num_terms=num_terms)
 
 
 # --------------------------------------------------------------------------

@@ -13,6 +13,8 @@
  *                               wavefront-error sums)
  *   k_zernike_moments<ROWS>     per-chunk Gram matrix of [OPD, Fringe Zernike terms] from a grid
  *                               trace's per-ray opd / status; k_reduce_zernike adds the chunks
+ *   k_aim_chief                 chief-ray aiming: the Newton iteration of rt_aim.cuh, one thread
+ *                               per field
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
  * The surface table (n_ifc x rt_surface_desc + n_wvl x n_ifc indices) is staged
@@ -34,6 +36,7 @@
 #include "rt_lean.cuh"
 #include "rt_grid.cuh"
 #include "rt_zernike.cuh"
+#include "rt_aim.cuh"
 
 using namespace b200rt;
 
@@ -1252,6 +1255,24 @@ k_chief_ref_focus(const rt_surface_desc *__restrict__ g_surfs, const double *__r
     }
 }
 
+/* chief-ray aiming of every field of a grid (rt_grid_aim_chief): aim_chief_ray of rt_aim.cuh, one
+ * thread per field, the table read from global memory as in k_chief_ref */
+__global__ void k_aim_chief(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                            int n_ifc, GridDev G, int n_fields, int stop, int wi,
+                            const double *__restrict__ g_wvl, rt_opts o, double h, double tol, int max_iter,
+                            double *__restrict__ aim_out, int32_t *__restrict__ term_out)
+{
+    const int f = blockIdx.x*blockDim.x + threadIdx.x;
+    if (f >= n_fields) return;
+    double ax, ay;
+    int iters;
+    const int term = aim_chief_ray(g_surfs, g_n + (int64_t)wi*n_ifc, g_wvl[wi], G, f, stop, o, h, tol, max_iter,
+                                   ax, ay, iters);
+    aim_out[f*2 + 0] = ax;
+    aim_out[f*2 + 1] = ay;
+    if (term_out) term_out[f] = term;
+}
+
 /* fp64 FMA microbenchmark: 8 independent chains per thread */
 __global__ void __launch_bounds__(256) k_dfma_peak(double *out, int iters, double a, double b)
 {
@@ -1926,6 +1947,34 @@ int rt_grid_chief_ref(const rt_table *t, rt_grid *g, int32_t wvl_idx, double *re
     k_chief_ref<<<blocks, threads, 0, (cudaStream_t)stream>>>(t->d_surfs, t->d_n, t->n_ifc, grid_dev(g),
                                                               g->n_fields, g->pupil_kind, wvl_idx, t->d_wvl,
                                                               o, g->d_ref_img, ref_out);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+int rt_grid_aim_chief(const rt_table *t, const rt_grid *g, int32_t stop, int32_t wvl_idx, double h, double tol,
+                      int32_t max_iter, double *aim_out, int32_t *term_out, void *stream)
+{
+    if (!t || !g) return fail(RT_ERR_INVALID, "rt_grid_aim_chief: table and grid are required");
+    if (!aim_out) return fail(RT_ERR_INVALID, "rt_grid_aim_chief: aim_out is required");
+    if (!(std::isfinite(h) && h > 0.0)) return fail(RT_ERR_INVALID, "rt_grid_aim_chief: h must be finite and positive");
+    if (!(std::isfinite(tol) && tol > 0.0))
+        return fail(RT_ERR_INVALID, "rt_grid_aim_chief: tol must be finite and positive");
+    if (max_iter < 0) return fail(RT_ERR_INVALID, "rt_grid_aim_chief: max_iter must not be negative");
+    if (g->pupil_kind != RT_PUPIL_EPD)
+        return fail(RT_ERR_UNSUPPORTED, "rt_grid_aim_chief: only 'epd' pupils (RT_PUPIL_EPD) are aimed on the device");
+    if (t->device != g->device) return fail(RT_ERR_INVALID, "rt_grid_aim_chief: table and grid on different devices");
+    if (stop < 1 || stop > t->n_ifc - 2) return fail(RT_ERR_INVALID, "rt_grid_aim_chief: stop must be in 1 ... n_ifc - 2");
+    if (wvl_idx < 0 || wvl_idx >= t->n_wvl) return fail(RT_ERR_INVALID, "rt_grid_aim_chief: wvl_idx out of range");
+    if (g->n_fields == 0) return RT_OK;
+    DeviceGuard guard(t->device);
+    rt_opts o;     /* cuda_bundle_fn's trace: first_surf 1, apertures not checked, intersect_obj on */
+    o.eps = 1.0e-12; o.pt_inside_fuzz = -1.0; o.check_apertures = 0; o.intersect_obj = 1;
+    o.filter_out_phantoms = 0; o.first_surf = 1; o.last_surf = stop; o.wvl_idx = wvl_idx;
+    const int threads = 32, blocks = (g->n_fields + threads - 1)/threads;
+    k_aim_chief<<<blocks, threads, 0, (cudaStream_t)stream>>>(t->d_surfs, t->d_n, t->n_ifc, grid_dev(g), g->n_fields,
+                                                              stop, wvl_idx, t->d_wvl, o, h, tol, max_iter, aim_out,
+                                                              term_out);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RT_OK;

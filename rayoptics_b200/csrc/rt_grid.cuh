@@ -82,6 +82,19 @@ __device__ __forceinline__ void grid_start_ray_at(const GridDev &G, int pupil_ki
     if (d0.z*(double)G.flip_z_dir < 0) { d0.x = -d0.x; d0.y = -d0.y; d0.z = -d0.z; }
 }
 
+/* the start ray of grid_start_ray_at<false> for RT_PUPIL_EPD without vignetting, aimed at
+ * (aim_x, aim_y) in place of the field's aim: the same expressions (rt_aim.cuh's trial rays) */
+__device__ __forceinline__ void epd_start_ray_aimed(const GridDev &G, int f, double pupx, double pupy,
+                                                    double aim_x, double aim_y, Vec3 &p0, Vec3 &d0)
+{
+    const rt_field_desc &F = G.fields[f];
+    p0.x = F.pt0[0]; p0.y = F.pt0[1]; p0.z = F.pt0[2];
+    Vec3 pt1 = {G.eprad*pupx + aim_x, G.eprad*pupy + aim_y, G.z_pupil};
+    Vec3 dv = {pt1.x - p0.x, pt1.y - p0.y, pt1.z - p0.z};
+    d0 = normalize3(dv);
+    if (d0.z*(double)G.flip_z_dir < 0) { d0.x = -d0.x; d0.y = -d0.y; d0.z = -d0.z; }
+}
+
 template <bool LEAN>
 __device__ __forceinline__ void grid_start_ray(const GridDev &G, int pupil_kind, int f, int64_t loc,
                                                Vec3 &p0, Vec3 &d0)

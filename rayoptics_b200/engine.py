@@ -777,6 +777,23 @@ def zernike_statistics(summary, wvl_sys, n_terms):
     return out
 
 
+def aim_chief_rays(table, grid, stop, wvl_idx, h, tol=1e-13, max_iter=30):
+    """``rt_grid_aim_chief``: the aim point of every field of a PupilGrid ('epd' pupil), found on the
+    device by the Newton iteration of ``vigcalc.aim_chief_ray`` (csrc/rt_aim.cuh) at row ``wvl_idx``
+    of the table with stop interface ``stop`` and forward-difference step ``h``.  Returns the device
+    tensors ``aim`` ``[n_fields, 2]`` float64 (the x == 0 rule of ``aim_chief_ray`` not applied) and
+    ``term`` ``[n_fields]`` int32 (``rt_aim_term``).  One launch, asynchronous on the current CUDA
+    stream; the grid's field records are not changed."""
+    lib = _abi.load_library()
+    device = torch.device('cuda', table.device)
+    aim = torch.empty((grid.n_fields, 2), dtype=torch.float64, device=device)
+    term = torch.empty(grid.n_fields, dtype=torch.int32, device=device)
+    with torch.cuda.device(device):
+        _abi.check(lib.rt_grid_aim_chief(table.handle, grid.handle, int(stop), int(wvl_idx), float(h), float(tol),
+                                         int(max_iter), _ptr(aim), _ptr(term), _stream_ptr(device)))
+    return aim, term
+
+
 def measure_fp64_peak(device=0):
     """TFLOP/s of the fp64 vector pipe (DFMA microbenchmark in the library)."""
     lib = _abi.load_library()

@@ -293,6 +293,47 @@ def aim_all_fields_batched(opt_model, bundle_fn=None, wvl=None, tol=1e-13, max_i
     return [f.aim_info for f in fields]
 
 
+def aim_fields_on_device(opt_model, fields, wvl=None, table=None, device=0, tol=1e-13, max_iter=30):
+    """``aim_all_fields_batched`` for the given ``Field`` objects with the whole iteration on the
+    device: one ``rt_grid_aim_chief`` launch (one thread per field, csrc/rt_aim.cuh) on the records
+    of ``grid_fields_of`` and one small copy back, then the ``fld.x == 0`` rule.  Sets
+    ``fld.aim_info``; returns the list.  A floating stop gives (0, 0) without a launch.  The
+    iteration is ``aim_chief_ray``'s with its own 2x2 solve (DESIGN.md section 4): on-meridian fields
+    get the aim points of ``aim_all_fields_batched`` bit for bit.  'epd' pupils only: wide-angle fields
+    and angular pupils raise NotImplementedError."""
+    from . import engine as E
+    from .analyses import _table_for
+    from .opticalspec import grid_fields_of
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    fields = list(fields)
+    stop = sm.stop_surface
+    if stop is None or not fields:
+        for fld in fields:
+            fld.aim_info = np.array([0., 0.])
+        return [f.aim_info for f in fields]
+    if _wide(opt_model):
+        raise NotImplementedError('aim_fields_on_device: wide-angle fields need the real entrance pupil search; '
+                                  'use vigcalc.aim_all_fields_batched (wideangle.aim_wide_angle_fields)')
+    recs, eprad, z_pupil = grid_fields_of(opt_model, fields)
+    if recs[0]['pupil_kind'] != 0:
+        raise NotImplementedError('aim_fields_on_device: angular pupils are not aimed on the device; '
+                                  'use vigcalc.aim_all_fields_batched or aim_chief_ray')
+    tab = _table_for(opt_model, table, device)
+    wvl = osp.spectral_region.central_wvl if wvl is None else wvl
+    wi = tab.wvl_index(wvl)
+    h = 1e-4*max(1.0, osp.fod.enp_radius)
+    grid = E.PupilGrid(recs, [wi], [0.0], [0.0], eprad, z_pupil, apply_vignetting=False,
+                       flip_z_dir=sm.z_dir[0], device=tab.device)
+    aim, _ = E.aim_chief_rays(tab, grid, stop, wi, h, tol, max_iter)
+    x = aim.cpu().numpy()                        # one small copy; waits
+    grid.close()
+    for i, fld in enumerate(fields):
+        if fld.x == 0.0:
+            x[i, 0] = 0.0
+        fld.aim_info = x[i].copy()
+    return [f.aim_info for f in fields]
+
+
 def set_clear_apertures_batched(opt_model, bundle_fn=None, wvl=None, avoid_list=None,
                                 include_list=None):
     """``set_clear_apertures`` (raytr/vigcalc.py:45-80) with the 5 boundary rays of all
