@@ -78,6 +78,19 @@ def test_planes_equal_single_focus_traces_partial_range(name):
     check_planes(name, 48, (2, 2))                    # empty range: identities
 
 
+@pytest.mark.parametrize('name', ['dblgauss', 'threemir'])
+def test_planes_between_sm_count_and_summary_ctas(name):
+    """num 227: 202 chunks per tile, more than the SMs but no more than the CTAs of the summary launch
+    (lean dblgauss: 3 per SM; general threemir: 2), so both launches keep per-chunk records.  Only a
+    range that cuts tiles tells that regime from work items."""
+    opm, tab, grid, wi = setup(name, 227)
+    n, cpt = grid.n_chunks, grid.chunks_per_tile
+    grid.close()
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    assert sms < cpt <= 2*sms
+    check_planes(name, 227, (3, n - 5))
+
+
 @pytest.mark.parametrize('name', MODELS)
 def test_chief_ref_focus(name):
     """plane k: the chief ray of rt_grid_chief_ref, defocused to foc[k] with p + (foc/d_z) d"""
