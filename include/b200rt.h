@@ -46,6 +46,8 @@ extern "C" {
 #define RT_WFE_DOUBLES 24    /* per-tile wavefront-error record of rt_trace_grid_wfe */
 #define RT_ZERN_DOUBLES 752  /* per-tile Zernike moments record of rt_grid_zernike */
 #define RT_ZERN_MAX_TERMS 37 /* Fringe Zernike terms of rt_grid_zernike */
+#define RT_MTF_MAX_RAYS 1024 /* pupil samples per side of rt_grid_pupil_function / rt_grid_mtf */
+#define RT_MTF_DOUBLES 8     /* per-tile record of rt_grid_mtf */
 
 /* error codes (function return values) */
 enum rt_error {
@@ -449,6 +451,30 @@ enum rt_aim_term {
 int rt_grid_aim_chief(const rt_table *table, const rt_grid *grid, int32_t stop, int32_t wvl_idx,
                       double h, double tol, int32_t max_iter, double *aim_out, int32_t *term_out,
                       void *stream);
+
+/* ---- diffraction MTF (ABI 6, additive): the pupil function of every tile of a grid trace and its
+ * autocorrelation along the two pupil axes (csrc/rt_mtf.cuh; DESIGN.md section 4).  The grid must be
+ * a product grid (paired = 0) without apply_vignetting with nx = ny = n <= RT_MTF_MAX_RAYS; the whole
+ * grid is processed (the autocorrelation needs every ray of a tile).  status / opd: DEVICE per-ray
+ * arrays of an rt_trace_grid over all chunks (opd in system units); ray (i, j) of tile t is entry
+ * t*n*n + i*n + j, at relative pupil coordinates (x, y) = (pupil_x[i], pupil_y[j]) of its field.  A
+ * ray is used when its status is 0 and x*x + y*y <= 1.  RT_ERR_INVALID before any device work for a
+ * bad grid or a NULL pointer.  One launch each on `stream`. */
+/* wvl_sys: DEVICE [n_tiles] wavelength of each tile in system units.  pupil, pupil_t: DEVICE
+ * [n_tiles][n][n] complex128 (re, im): pupil[t][i][j] = P = exp(2 pi i opd/wvl_sys) of a used ray
+ * (sincospi(2.0*w), w = opd/wvl_sys rounded once), +0.0 otherwise; pupil_t[t][j][i] = the same value. */
+int rt_grid_pupil_function(const rt_grid *grid, const int32_t *status, const double *opd, const double *wvl_sys,
+                           double *pupil, double *pupil_t, void *stream);
+/* pupil, pupil_t: rt_grid_pupil_function's outputs; status: the trace's.  acf_x, acf_y: DEVICE
+ * [n_tiles][n] complex128: acf_x[t][k] = Cx(k) = sum over i < n-k and all j of P[i+k][j]*conj(P[i][j]),
+ * acf_y the same along j.  record: DEVICE [n_tiles][RT_MTF_DOUBLES]:
+ *   0-4 status-class counts of every ray (as the wavefront-error record)   5 n_used   6, 7 Re, Im S
+ * with S = sum of P.  Sum order: products a*conj(b) as re = ar*br + ai*bi, im = ai*br - ar*bi, every
+ * product rounded once; each line (fixed j for Cx and S, fixed i for Cy) added in increasing index
+ * along the other axis from +0.0; the line sums added in line order from +0.0.  Bit-reproducible,
+ * independent of the launch shape. */
+int rt_grid_mtf(const rt_grid *grid, const int32_t *status, const double *pupil, const double *pupil_t,
+                double *acf_x, double *acf_y, double *record, void *stream);
 
 /* ---- misc */
 const char *rt_last_error(void);

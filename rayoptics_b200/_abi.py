@@ -20,6 +20,8 @@ RT_MAX_FOCUS = 64
 RT_WFE_DOUBLES = 24
 RT_ZERN_DOUBLES = 752
 RT_ZERN_MAX_TERMS = 37
+RT_MTF_MAX_RAYS = 1024
+RT_MTF_DOUBLES = 8
 
 # enum rt_profile
 PROFILE_IDS = {'Spherical': 0, 'Conic': 1, 'EvenPolynomial': 2,
@@ -124,7 +126,8 @@ EXPORTS = ['rt_table_create', 'rt_table_destroy', 'rt_table_dims', 'rt_table_set
            'rt_last_error', 'rt_abi_version', 'rt_chunk_rays', 'rt_launch_count', 'rt_measure_fp64_peak', 'rt_measure_fp64_latency',
            'rt_selftest_division', 'rt_grid_chief_ref_focus', 'rt_grid_focus_scratch_bytes',
            'rt_trace_grid_focus', 'rt_grid_wfe_scratch_bytes', 'rt_trace_grid_wfe', 'rt_combine_wfe',
-           'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike', 'rt_grid_aim_chief']
+           'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike', 'rt_grid_aim_chief',
+           'rt_grid_pupil_function', 'rt_grid_mtf']
 
 _lib = None
 
@@ -200,6 +203,10 @@ def load_library():
     lib.rt_combine_zernike.restype = i32
     lib.rt_grid_aim_chief.argtypes = [vp, vp, i32, i32, C.c_double, C.c_double, i32, vp, vp, vp]
     lib.rt_grid_aim_chief.restype = i32
+    lib.rt_grid_pupil_function.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.rt_grid_pupil_function.restype = i32
+    lib.rt_grid_mtf.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.rt_grid_mtf.restype = i32
     lib.rt_last_error.restype = C.c_char_p
     lib.rt_abi_version.restype = i32
     lib.rt_chunk_rays.restype = i32

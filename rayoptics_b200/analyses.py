@@ -364,12 +364,14 @@ def _wfe_sums_host(spec, status, opd):
 
 
 def wavefront_grid_args(opt_model, table, num_rays, fields, wvls, foc, image_pt_2d=None, image_delta=None,
-                        backend=None):
+                        backend=None, ref_wvl_for_image_pt=None):
     """``(args, kw)`` of the PupilGridSpec / PupilGrid that ``wavefront_error`` traces: the chief rays
     and reference spheres of all tiles (one ``waveabr.setup_tiles`` call), each field's ``RayGrid``
-    pupil samples, no vignetting applied"""
+    pupil samples, no vignetting applied.  ``ref_wvl_for_image_pt``: refer every wavelength to that
+    wavelength's chief-ray image point (``setup_tiles``); by default each its own"""
     sm = opt_model.seq_model
     wave, ref_img, _ = W.setup_tiles(opt_model, table, fields, wvls, foc, image_pt_2d, image_delta,
+                                     ref_wvl_for_image_pt=ref_wvl_for_image_pt,
                                      chief_tracer=None if backend is None else backend.chief_rays)
     pupils = [_wavefront_pupil(opt_model, fld, num_rays) for fld in fields]
     recs, eprad, z_pupil = grid_fields_of(opt_model, fields)
@@ -513,6 +515,174 @@ def zernike_fit(opt_model, num_rays=64, num_terms=37, fields=None, wvls=None, fo
     lam = np.array([[opt_model.nm_to_sys_units(w) for w in wvls]]*len(fields)).ravel()
     stats = E.zernike_statistics(summ_host, lam, num_terms)
     return ZernikeFit(stats, summ_host, ref_img, num_rays, num_terms, len(fields), len(wvls))
+
+
+class MTF:
+    """Result of ``mtf``, per field and wavelength.  Slices along the pupil axes: for fields on the y
+    axis ``*_y`` is tangential and ``*_x`` sagittal.
+
+    ``otf_x``, ``otf_y`` ``[n_fields, n_wvls, N]`` complex: the OTF against the pupil shift k =
+    0 ... N-1 (``otf[..., 0]`` = 1); ``mtf_x``, ``mtf_y``: their moduli; ``freq_x``, ``freq_y``
+    ``[n_fields, n_wvls, N]``: the frequency of each shift in cycles per system unit (NaN for tiles
+    with an infinite reference sphere); ``cutoff`` ``[n_fields, n_wvls]``: 2 r_xp/(lambda |R|);
+    ``strehl``: |sum P|^2/n_used^2 at the reference image point; ``n_used`` and the ray counts
+    ``n_ok``, ``n_missed``, ``n_tir``, ``n_blocked``, ``n_other``; ``ref_img`` ``[n_fields, n_wvls,
+    2]``; ``acf_x``, ``acf_y``, ``record``: the device's unnormalised autocorrelations and records.
+    With ``freqs`` ``[K]``: ``otf_x_at``, ``otf_y_at``, ``mtf_x_at``, ``mtf_y_at`` ``[n_fields,
+    n_wvls, K]``; polychromatic: ``poly_x``, ``poly_y`` ``[n_fields, K]`` and the weights ``wts``."""
+
+    def __init__(self, **kw):
+        for k, v in kw.items():
+            setattr(self, k, v)
+
+
+def _mtf_host(spec, status, opd, lam):
+    """``(acf_x, acf_y, record)`` of traced rays, formed on the host (the ``backend=`` test seam; the
+    device forms them in ``rt_grid_pupil_function`` and ``rt_grid_mtf``)"""
+    n, per = spec.nx, spec.rays_per_tile
+    acf_x = np.zeros((spec.n_tiles, n), dtype=np.complex128)
+    acf_y = np.zeros((spec.n_tiles, n), dtype=np.complex128)
+    rec = np.zeros((spec.n_tiles, E.RT_MTF_DOUBLES))
+    for t in range(spec.n_tiles):
+        f = t//spec.n_wvls
+        gx, gy = np.meshgrid(spec.pupil_x[f], spec.pupil_y[f], indexing='ij')
+        st, w = status[t*per:(t + 1)*per].reshape(n, n), opd[t*per:(t + 1)*per].reshape(n, n)
+        P = E.pupil_function_host(st, w, gx, gy, lam[t])
+        acf_x[t], acf_y[t], S = E.mtf_sums_host(P)
+        cls = np.where((st >= 0) & (st <= 3), st, 4).ravel()
+        rec[t, 0:5] = np.bincount(cls, minlength=5)[:5]
+        rec[t, 5] = ((st == 0) & (gx*gx + gy*gy <= 1.0)).sum()
+        rec[t, 6:8] = S.real, S.imag
+    return acf_x, acf_y, rec
+
+
+def mtf_frequencies(pupil, wave, lam, exp_radius):
+    """``(freq [n_tiles, N], cutoff [n_tiles])`` of the shifts k = 0 ... N-1 along one pupil axis:
+    nu_k = k*delta*r_xp/(lambda*|R|), delta = (pupil[-1] - pupil[0])/(N - 1) (relative pupil units,
+    per field), R the tile's reference-sphere radius; NaN for tiles with an infinite reference sphere.
+    ``pupil`` ``[n_fields, N]``; ``wave`` ``[n_fields, n_wvls, RT_WAVE_DOUBLES]``; ``lam`` ``[n_tiles]``
+    in system units."""
+    pupil = np.asarray(pupil, dtype=np.float64)
+    nf, n = pupil.shape
+    nw = wave.shape[1]
+    delta = (pupil[:, -1] - pupil[:, 0])/(n - 1) if n > 1 else np.zeros(nf)
+    R = np.abs(wave[:, :, 20]).ravel()
+    scale = np.where(wave[:, :, 21].ravel() == 0.0, np.nan, exp_radius/(np.asarray(lam)*R))
+    freq = np.arange(n)[None, :]*np.repeat(delta, nw)[:, None]*scale[:, None]
+    return freq, 2.0*scale
+
+
+def otf_at(freqs, freq, otf, cutoff):
+    """complex OTF ``[n_tiles, K]`` at the frequencies ``freqs`` (>= 0), linear in nu between the
+    native shifts ``freq`` ``[n_tiles, N]``; 0 past the last shift and past the tile's cutoff, NaN
+    where the tile's frequencies are NaN"""
+    freqs = np.asarray(freqs, dtype=np.float64).reshape(-1)
+    out = np.empty((freq.shape[0], len(freqs)), dtype=np.complex128)
+    for t in range(freq.shape[0]):
+        if not np.isfinite(freq[t]).all() or not np.isfinite(cutoff[t]):
+            out[t] = np.nan
+            continue
+        v = (np.interp(freqs, freq[t], otf[t].real, right=0.0)
+             + 1j*np.interp(freqs, freq[t], otf[t].imag, right=0.0))
+        out[t] = np.where(freqs > cutoff[t], 0.0, v)
+    return out
+
+
+def polychromatic_mtf(otf, wts):
+    """|sum_w wts[w]*otf[..., w, :]|/sum wts: ``otf`` ``[n_fields, n_wvls, K]`` complex at common
+    frequencies, referred to one image point -> ``[n_fields, K]``"""
+    wts = np.asarray(wts, dtype=np.float64)
+    return np.abs(np.einsum('fwk,w->fk', np.asarray(otf), wts))/wts.sum()
+
+
+def mtf(opt_model, num_rays=64, fields=None, wvls=None, foc=None, image_pt_2d=None, image_delta=None,
+        freqs=None, polychromatic=False, table=None, device=0, backend=None, **trace_kwargs):
+    """Diffraction MTF along the two pupil axes and the Strehl ratio of every field and wavelength,
+    from one grid trace.
+
+    The rays are those of ``zernike_fit`` (``RayGrid``'s: ``num_rays`` x ``num_rays`` samples over
+    the field's vignetting bounding box, no vignetting applied, apertures checked, the same chief ray
+    and reference sphere); a ray is used when its status is 0 and x^2 + y^2 <= 1.  On the device the
+    pupil function P = exp(2 pi i opd/lambda) of the used rays (0 elsewhere) is autocorrelated along
+    pupil x and y in a fixed order (``rt_grid_mtf``, DESIGN.md section 4); only the ``[n_tiles, N]``
+    autocorrelations and the ``[n_tiles, RT_MTF_DOUBLES]`` records come back.  OTF(k) = C(k)/C(0);
+    the frequency of shift k is ``mtf_frequencies``'; the Strehl ratio is |sum P|^2/n_used^2, the
+    discrete Fraunhofer PSF at the tile's reference image point over the unaberrated peak (tilt with
+    respect to that point counts against it; ``image_pt_2d`` / ``image_delta`` move the point).
+
+    The slices are along the pupil axes: for fields on the y axis ``y`` is tangential and ``x``
+    sagittal.  ``freqs``: frequencies (cycles per system unit, >= 0) at which the OTF is also
+    returned, interpolated linearly in nu.  ``polychromatic``: refer every wavelength to the chief-ray
+    image point of the central wavelength (which must be among ``wvls``) and return |sum w OTF(nu)| /
+    sum w at ``freqs`` (required), with w the model's spectral weights.  ``backend``: the CPU test seam
+    of ``RayGrid``.  ``trace_kwargs``: trace options (``check_apertures``, ...).  Returns an ``MTF``."""
+    if not 1 <= int(num_rays) <= E.RT_MTF_MAX_RAYS:
+        raise ValueError(f'num_rays must be 1 ... {E.RT_MTF_MAX_RAYS}')
+    if polychromatic and freqs is None:
+        raise ValueError('polychromatic=True needs freqs=')
+    if freqs is not None:
+        freqs = np.asarray(freqs, dtype=np.float64).reshape(-1)
+        if not (np.isfinite(freqs).all() and (freqs >= 0).all()):
+            raise ValueError('freqs must be finite and >= 0')
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    fields = list(osp.field_of_view.fields if fields is None else fields)
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    foc = osp.defocus.focus_shift if foc is None else foc
+    ref_wvl = None
+    if polychromatic:
+        ref_wvl = sm.central_wavelength()
+        if ref_wvl not in wvls:
+            raise ValueError('polychromatic=True needs the central wavelength among wvls')
+    nf, nw, n = len(fields), len(wvls), int(num_rays)
+    tab = None if backend is not None else _table_for(opt_model, table, device)
+    args, grid_kw = wavefront_grid_args(opt_model, tab, n, fields, wvls, foc, image_pt_2d, image_delta, backend,
+                                        ref_wvl_for_image_pt=ref_wvl)
+    lam = np.array([[opt_model.nm_to_sys_units(w) for w in wvls]]*nf).ravel()
+    trace_kwargs.setdefault('check_apertures', True)
+    if backend is not None:
+        spec = E.PupilGridSpec(*args, **grid_kw)
+        r = backend.trace_tile(opt_model, spec, True, trace_kwargs['check_apertures'])
+        acf_x, acf_y, rec = _mtf_host(spec, np.asarray(r['status']), np.asarray(r['opd']), lam)
+    else:
+        dev = torch.device('cuda', tab.device)
+        with torch.cuda.device(dev):
+            grid = E.PupilGrid(*args, device=tab.device, **grid_kw)
+            cx, cy, rec_d, _ = E.trace_grid_mtf(tab, grid, lam, **trace_kwargs)
+            host = torch.cat([torch.view_as_real(cx).reshape(-1), torch.view_as_real(cy).reshape(-1),
+                              rec_d.reshape(-1)]).cpu().numpy()       # one small copy; waits
+            grid.close()
+        m = grid.n_tiles*n*2
+        acf_x = host[:m].view(np.complex128).reshape(-1, n)
+        acf_y = host[m:2*m].view(np.complex128).reshape(-1, n)
+        rec = host[2*m:].reshape(-1, E.RT_MTF_DOUBLES)
+    wave = grid_kw['wave']
+    fod = opt_model['analysis_results']['parax_data'].fod
+    freq_x, cutoff = mtf_frequencies(args[2], wave, lam, fod.exp_radius)
+    freq_y, _ = mtf_frequencies(args[3], wave, lam, fod.exp_radius)
+    with np.errstate(invalid='ignore', divide='ignore'):
+        otf_x = acf_x/acf_x[:, :1].real                 # C(0) is real: every term of it is a*conj(a)
+        otf_y = acf_y/acf_y[:, :1].real
+        strehl = (rec[:, 6]**2 + rec[:, 7]**2)/rec[:, 5]**2
+    shape = (nf, nw)
+    out = dict(otf_x=otf_x.reshape(nf, nw, n), otf_y=otf_y.reshape(nf, nw, n),
+               mtf_x=np.abs(otf_x).reshape(nf, nw, n), mtf_y=np.abs(otf_y).reshape(nf, nw, n),
+               freq_x=freq_x.reshape(nf, nw, n), freq_y=freq_y.reshape(nf, nw, n),
+               cutoff=cutoff.reshape(shape), strehl=strehl.reshape(shape), acf_x=acf_x, acf_y=acf_y,
+               record=rec, ref_img=grid_kw['ref_img'], num_rays=n, n_fields=nf, n_wvls=nw, freqs=freqs,
+               polychromatic=bool(polychromatic))
+    for i, k in enumerate(E.MTF_RECORD[:6]):
+        out[k] = rec[:, i].reshape(shape)
+    if freqs is not None:
+        for ax, o, fq in (('x', otf_x, freq_x), ('y', otf_y, freq_y)):
+            at = otf_at(freqs, fq, o, cutoff).reshape(nf, nw, -1)
+            out[f'otf_{ax}_at'], out[f'mtf_{ax}_at'] = at, np.abs(at)
+        if polychromatic:
+            region = osp.spectral_region
+            wts = np.array([region.spectral_wts[list(region.wavelengths).index(w)] for w in wvls])
+            out['wts'] = wts
+            out['poly_x'] = polychromatic_mtf(out['otf_x_at'], wts)
+            out['poly_y'] = polychromatic_mtf(out['otf_y_at'], wts)
+    return MTF(**out)
 
 
 class FieldMap:

@@ -15,6 +15,8 @@
  *                               trace's per-ray opd / status; k_reduce_zernike adds the chunks
  *   k_aim_chief                 chief-ray aiming: the Newton iteration of rt_aim.cuh, one thread
  *                               per field
+ *   k_pupil_function, k_mtf     pupil function of a grid trace's per-ray opd / status, and its
+ *                               autocorrelation along both pupil axes (rt_mtf.cuh)
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
  * The surface table (n_ifc x rt_surface_desc + n_wvl x n_ifc indices) is staged
@@ -37,6 +39,7 @@
 #include "rt_grid.cuh"
 #include "rt_zernike.cuh"
 #include "rt_aim.cuh"
+#include "rt_mtf.cuh"
 
 using namespace b200rt;
 
@@ -1209,6 +1212,81 @@ __global__ void k_combine_zernike(const double *__restrict__ parts, int n_parts,
     combine_rows<ZernLayout>(parts, n_parts, n, out);
 }
 
+/* ---- diffraction MTF (rt_grid_pupil_function, rt_grid_mtf; rt_mtf.cuh).  Tiles of n x n rays,
+ * ray (i, j) at i*n + j. */
+#define RT_MTF_THREADS 256
+
+/* one thread per ray: the phasor into P[tile][i*n + j] and its transposed copy PT[tile][j*n + i],
+ * from which k_mtf reads the lines along y with coalesced loads */
+__global__ void __launch_bounds__(RT_MTF_THREADS)
+k_pupil_function(GridDev G, int64_t n_rays, const int32_t *__restrict__ status, const double *__restrict__ opd,
+                 const double *__restrict__ wvl_sys, MtfC *__restrict__ P, MtfC *__restrict__ PT)
+{
+    const int64_t r = (int64_t)blockIdx.x*blockDim.x + threadIdx.x;
+    if (r >= n_rays) return;
+    const int n = G.nx;
+    const int64_t tile = r/G.rays_per_tile, loc = r - tile*G.rays_per_tile;
+    const int64_t i = loc/n, j = loc - i*n;
+    const int f = (int)(tile/G.n_wvls);
+    const double x = G.pupil_x[(int64_t)f*n + i], y = G.pupil_y[(int64_t)f*n + j];
+    const MtfC p = mtf_used(status[r], x, y) ? mtf_phasor(opd[r], wvl_sys[tile]) : MtfC{0.0, 0.0};
+    P[r] = p;
+    PT[tile*G.rays_per_tile + j*n + i] = p;
+}
+
+/* One CTA per (tile, slot), slot = 0 ... 2n: slot k < n is Cx(k), n + k is Cy(k), 2n the tile's
+ * record.  A thread per line (strided over the CTA) adds its line in index order; thread 0 then adds
+ * the line sums in line order (rt_mtf.cuh).  Lines along x are the columns of P and lines along y
+ * the columns of PT, so a warp's loads are always 32 adjacent values.  No atomics, no scratch. */
+__global__ void __launch_bounds__(RT_MTF_THREADS)
+k_mtf(GridDev G, const int32_t *__restrict__ status, const MtfC *__restrict__ P, const MtfC *__restrict__ PT,
+      MtfC *__restrict__ acf_x, MtfC *__restrict__ acf_y, double *__restrict__ rec)
+{
+    __shared__ MtfC lines[RT_MTF_MAX_RAYS];
+    __shared__ int cnt[RT_MTF_THREADS][6];
+    const int n = G.nx;
+    const int64_t tile = blockIdx.x/(2*n + 1);
+    const int slot = (int)(blockIdx.x - tile*(2*n + 1));
+    const int64_t base = tile*G.rays_per_tile;
+    if (slot < 2*n) {
+        const bool ax = slot < n;
+        const int k = ax ? slot : slot - n;
+        const MtfC *src = (ax ? P : PT) + base;
+        for (int l = threadIdx.x; l < n; l += blockDim.x) lines[l] = mtf_line_shift(src + l, n, n, k);
+        __syncthreads();
+        if (threadIdx.x == 0) (ax ? acf_x : acf_y)[tile*n + k] = mtf_line_sum(lines, 1, n);
+        return;
+    }
+    /* the record: S = sum P (lines along x), the status classes and the used rays */
+    const int f = (int)(tile/G.n_wvls);
+    int c[6] = {0, 0, 0, 0, 0, 0};
+    for (int l = threadIdx.x; l < n; l += blockDim.x) {
+        lines[l] = mtf_line_sum(P + base + l, n, n);
+        const double y = G.pupil_y[(int64_t)f*n + l];
+        for (int i = 0; i < n; i++) {
+            const int st = status[base + (int64_t)i*n + l];
+            const int ck = (st >= 0 && st <= RT_RAY_BLOCKED) ? st : 4;
+#pragma unroll
+            for (int q = 0; q < 5; q++) c[q] += ck == q;          /* constant indices: c stays in registers */
+            c[5] += mtf_used(st, G.pupil_x[(int64_t)f*n + i], y);
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < 6; q++) cnt[threadIdx.x][q] = c[q];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int t = 1; t < blockDim.x; t++)
+#pragma unroll
+            for (int q = 0; q < 6; q++) c[q] += cnt[t][q];
+        const MtfC s = mtf_line_sum(lines, 1, n);
+        double *out = rec + tile*RT_MTF_DOUBLES;
+#pragma unroll
+        for (int q = 0; q < 6; q++) out[q] = (double)c[q];
+        out[6] = s.re;
+        out[7] = s.im;
+    }
+}
+
 /* chief rays of all fields: pupil (0, 0), no vignetting, apertures not checked, general
  * per-ray code on the global table (bit-identical to the lean loop by construction, and
  * n_fields rays do not need the specialised kernel).  One thread per field. */
@@ -2243,6 +2321,49 @@ int rt_combine_zernike(const double *parts, int32_t n_parts, int64_t n_tiles, do
     if (n_tiles == 0) return RT_OK;
     const int64_t n = n_tiles*RT_ZERN_DOUBLES;
     k_combine_zernike<<<(unsigned)((n + 255)/256), 256, 0, (cudaStream_t)stream>>>(parts, n_parts, n, out);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+/* the grid conditions of rt_grid_pupil_function / rt_grid_mtf */
+static int mtf_check_grid(const rt_grid *g, const char *fn)
+{
+    if (!g) return fail(RT_ERR_INVALID, "%s: grid is required", fn);
+    if (g->paired) return fail(RT_ERR_INVALID, "%s: needs a product grid (paired = 0)", fn);
+    if (g->apply_vignetting)
+        return fail(RT_ERR_INVALID, "%s: the pupil coordinates must not be vignetted (apply_vignetting = 0)", fn);
+    if (g->nx != g->ny) return fail(RT_ERR_INVALID, "%s: needs a square grid (nx = ny)", fn);
+    if (g->nx > RT_MTF_MAX_RAYS) return fail(RT_ERR_INVALID, "%s: nx exceeds RT_MTF_MAX_RAYS", fn);
+    return RT_OK;
+}
+
+int rt_grid_pupil_function(const rt_grid *g, const int32_t *status, const double *opd, const double *wvl_sys,
+                           double *pupil, double *pupil_t, void *stream)
+{
+    if (const int rc = mtf_check_grid(g, "rt_grid_pupil_function")) return rc;
+    if (!status || !opd || !wvl_sys || !pupil || !pupil_t)
+        return fail(RT_ERR_INVALID, "rt_grid_pupil_function: status, opd, wvl_sys, pupil and pupil_t are required");
+    DeviceGuard guard(g->device);
+    const int64_t n = g->n_rays;
+    k_pupil_function<<<(unsigned)((n + RT_MTF_THREADS - 1)/RT_MTF_THREADS), RT_MTF_THREADS, 0, (cudaStream_t)stream>>>(
+        grid_dev(g), n, status, opd, wvl_sys, (MtfC *)pupil, (MtfC *)pupil_t);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+int rt_grid_mtf(const rt_grid *g, const int32_t *status, const double *pupil, const double *pupil_t,
+                double *acf_x, double *acf_y, double *record, void *stream)
+{
+    if (const int rc = mtf_check_grid(g, "rt_grid_mtf")) return rc;
+    if (!status || !pupil || !pupil_t || !acf_x || !acf_y || !record)
+        return fail(RT_ERR_INVALID, "rt_grid_mtf: status, pupil, pupil_t, acf_x, acf_y and record are required");
+    DeviceGuard guard(g->device);
+    const int n = g->nx;
+    const int threads = n >= RT_MTF_THREADS ? RT_MTF_THREADS : (n + 31)/32*32;
+    k_mtf<<<(unsigned)(g->n_tiles*(2*n + 1)), threads, 0, (cudaStream_t)stream>>>(
+        grid_dev(g), status, (const MtfC *)pupil, (const MtfC *)pupil_t, (MtfC *)acf_x, (MtfC *)acf_y, record);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RT_OK;

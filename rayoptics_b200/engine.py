@@ -20,7 +20,7 @@ import torch
 
 from . import _abi
 from ._abi import (rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES, RT_WFE_DOUBLES,
-                   RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS)
+                   RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS, RT_MTF_DOUBLES, RT_MTF_MAX_RAYS)
 
 SUMMARY_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other',
                   'sum_x', 'sum_y', 'sum_xx', 'sum_yy', 'sum_xy',
@@ -792,6 +792,118 @@ def aim_chief_rays(table, grid, stop, wvl_idx, h, tol=1e-13, max_iter=30):
         _abi.check(lib.rt_grid_aim_chief(table.handle, grid.handle, int(stop), int(wvl_idx), float(h), float(tol),
                                          int(max_iter), _ptr(aim), _ptr(term), _stream_ptr(device)))
     return aim, term
+
+
+# --- diffraction MTF (rt_grid_pupil_function, rt_grid_mtf; the sums of csrc/rt_mtf.cuh) -----------
+MTF_RECORD = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other', 'n_used', 'sum_re', 'sum_im')
+
+
+def _ray_tensor(t, dt, n, name):
+    if not (torch.is_tensor(t) and t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n):
+        raise ValueError(f'{name} must be a contiguous {dt} CUDA tensor of {n} entries')
+
+
+def grid_pupil_function(grid, status, opd, wvl_sys):
+    """``rt_grid_pupil_function``: ``(pupil, pupil_t)``, ``[n_tiles, n, n]`` complex128 device tensors
+    of the pupil function exp(2 pi i opd/wvl_sys) of every tile of a square product PupilGrid without
+    vignetting (0 where a ray is not used: status != 0 or x^2 + y^2 > 1), ``pupil_t`` transposed in
+    each tile.  ``status`` (int32), ``opd`` (float64, system units): the per-ray device tensors of a
+    grid trace over all chunks; ``wvl_sys``: the wavelength in system units, a scalar or one value per
+    tile.  Asynchronous on the current CUDA stream."""
+    lib = _abi.load_library()
+    _ray_tensor(status, torch.int32, grid.n_rays, 'status')
+    _ray_tensor(opd, torch.float64, grid.n_rays, 'opd')
+    device = status.device
+    lam = np.broadcast_to(np.asarray(wvl_sys, dtype=np.float64).reshape(-1), (grid.n_tiles,))
+    lam = torch.tensor(lam, device=device)
+    shape = (grid.n_tiles, grid.nx, grid.ny)
+    pupil = torch.empty(shape, dtype=torch.complex128, device=device)
+    pupil_t = torch.empty(shape, dtype=torch.complex128, device=device)
+    with torch.cuda.device(device):
+        _abi.check(lib.rt_grid_pupil_function(grid.handle, _ptr(status), _ptr(opd), _ptr(lam), _ptr(pupil),
+                                              _ptr(pupil_t), _stream_ptr(device)))
+    pupil._keep = (status, opd, lam)           # must outlive the asynchronous launch
+    return pupil, pupil_t
+
+
+def grid_mtf(grid, status, pupil, pupil_t):
+    """``rt_grid_mtf``: ``(acf_x, acf_y, record)`` of ``grid_pupil_function``'s outputs:
+    ``[n_tiles, n]`` complex128 autocorrelations along pupil x and y against the shift k, and the
+    ``[n_tiles, RT_MTF_DOUBLES]`` record (``MTF_RECORD``: status counts, n_used, Re / Im of sum P).
+    Asynchronous on the current CUDA stream."""
+    lib = _abi.load_library()
+    _ray_tensor(status, torch.int32, grid.n_rays, 'status')
+    for t, name in ((pupil, 'pupil'), (pupil_t, 'pupil_t')):
+        _ray_tensor(t, torch.complex128, grid.n_rays, name)
+    device = status.device
+    acf_x = torch.empty((grid.n_tiles, grid.nx), dtype=torch.complex128, device=device)
+    acf_y = torch.empty((grid.n_tiles, grid.nx), dtype=torch.complex128, device=device)
+    rec = torch.empty((grid.n_tiles, RT_MTF_DOUBLES), dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        _abi.check(lib.rt_grid_mtf(grid.handle, _ptr(status), _ptr(pupil), _ptr(pupil_t), _ptr(acf_x),
+                                   _ptr(acf_y), _ptr(rec), _stream_ptr(device)))
+    rec._keep = (status, pupil, pupil_t)
+    return acf_x, acf_y, rec
+
+
+def trace_grid_mtf(table, grid, wvl_sys, res=None, **kwargs):
+    """Autocorrelations of the pupil functions of every tile of a square PupilGrid built with
+    ``wave=`` records: ``trace_grid`` over all chunks with the ``opd`` and ``status`` outputs into
+    device buffers (``res``: an optional BundleResult with both, which keeps them), then
+    ``grid_pupil_function`` and ``grid_mtf`` -- three launches.  Returns ``(acf_x, acf_y, record,
+    pupil)`` device tensors.  Trace defaults as ``trace_grid``."""
+    if res is None:
+        res = BundleResult(grid.n_rays, table.n_ifc, torch.device('cuda', table.device), ('opd', 'status'))
+    elif res.opd is None or res.status is None:
+        raise ValueError('res needs the opd and status outputs')
+    trace_grid(table, grid, 0, grid.n_chunks, summary=False, res=res, **kwargs)
+    pupil, pupil_t = grid_pupil_function(grid, res.status, res.opd, wvl_sys)
+    acf_x, acf_y, rec = grid_mtf(grid, res.status, pupil, pupil_t)
+    rec._keep = (rec._keep, res)
+    return acf_x, acf_y, rec, pupil
+
+
+def pupil_function_host(status, opd, x, y, wvl_sys):
+    """numpy pupil function of one tile: ``status`` / ``opd`` ``[n, n]``, ``x`` / ``y`` the relative
+    pupil coordinates broadcast to ``[n, n]``; exp(2 pi i (w - rint w)), w = opd/wvl_sys, where
+    status is 0 and x^2 + y^2 <= 1, else 0.  Within an ulp or two of the device's sincospi."""
+    used = (np.asarray(status) == 0) & (x*x + y*y <= 1.0)
+    with np.errstate(invalid='ignore'):
+        w = np.asarray(opd, dtype=np.float64)/wvl_sys
+        r = 2.0*np.pi*(w - np.rint(w))
+        p = np.cos(r) + 1j*np.sin(r)
+    return np.where(used, p, 0.0 + 0.0j)
+
+
+def _line_sums_in_order(v):
+    """``v [n_lines, ...]`` real: the sum over axis 0 from +0.0 in increasing index (a sequential
+    chain, not numpy's pairwise sum)"""
+    acc = np.zeros(v.shape[1:])
+    for row in v:
+        acc = acc + row
+    return acc
+
+
+def _autocorr_host(P):
+    """Cx of ``P [n, n]`` in the order of rt_mtf.cuh: chains along axis 0 for every (k, line j) at
+    once (row i of every chain added at step i), then the lines of each k in order"""
+    n = P.shape[0]
+    pr, pi = np.ascontiguousarray(P.real), np.ascontiguousarray(P.imag)
+    acc_r, acc_i = np.zeros((n, n)), np.zeros((n, n))          # [k, j]
+    for i in range(n):
+        ar, ai, br, bi = pr[i:], pi[i:], pr[i], pi[i]            # a = P[i + k], b = P[i], k < n - i
+        acc_r[:n - i] = acc_r[:n - i] + (ar*br + ai*bi)
+        acc_i[:n - i] = acc_i[:n - i] + (ai*br - ar*bi)
+    return _line_sums_in_order(acc_r.T) + 1j*_line_sums_in_order(acc_i.T)
+
+
+def mtf_sums_host(P):
+    """``(acf_x [n], acf_y [n], S)`` of one tile's ``[n, n]`` complex128 pupil function (x outer), bit
+    for bit in the order of ``rt_grid_mtf`` (the ``backend=`` seam of ``analyses.mtf``)"""
+    P = np.asarray(P, dtype=np.complex128)
+    s_lines = _line_sums_in_order(P.real) + 1j*_line_sums_in_order(P.imag)       # line j: along i
+    S = complex(_line_sums_in_order(s_lines.real[:, None])[0], _line_sums_in_order(s_lines.imag[:, None])[0])
+    return _autocorr_host(P), _autocorr_host(P.T), S
 
 
 def measure_fp64_peak(device=0):
