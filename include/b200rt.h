@@ -48,6 +48,7 @@ extern "C" {
 #define RT_ZERN_MAX_TERMS 37 /* Fringe Zernike terms of rt_grid_zernike */
 #define RT_MTF_MAX_RAYS 1024 /* pupil samples per side of rt_grid_pupil_function / rt_grid_mtf */
 #define RT_MTF_DOUBLES 8     /* per-tile record of rt_grid_mtf */
+#define RT_SPHERE_DOUBLES 8  /* per-(plane, tile) reference-sphere record of rt_trace_grid_opd_focus */
 
 /* error codes (function return values) */
 enum rt_error {
@@ -475,6 +476,34 @@ int rt_grid_pupil_function(const rt_grid *grid, const int32_t *status, const dou
  * independent of the launch shape. */
 int rt_grid_mtf(const rt_grid *grid, const int32_t *status, const double *pupil, const double *pupil_t,
                 double *acf_x, double *acf_y, double *record, void *stream);
+/* rt_grid_mtf at listed shifts only.  shifts: DEVICE [n_shifts], each in [0, n-1], any order,
+ * duplicates allowed (an entry outside that range gives NaN).  acf_x, acf_y: DEVICE
+ * [n_tiles][n_shifts] complex128; entry m is bit for bit rt_grid_mtf's entry shifts[m].  record: as
+ * rt_grid_mtf.  n_shifts = 0 computes the record alone (shifts, acf_x and acf_y may be NULL).  One
+ * launch on `stream`; RT_ERR_INVALID before any device work as rt_grid_mtf, and for n_shifts < 0. */
+int rt_grid_mtf_shifts(const rt_grid *grid, const int32_t *status, const double *pupil, const double *pupil_t,
+                       const int32_t *shifts, int32_t n_shifts, double *acf_x, double *acf_y,
+                       double *record, void *stream);
+
+/* ---- OPD at many reference spheres (ABI 6, additive): one trace of chunks [chunk_begin, chunk_end)
+ * of a grid with rt_grid_spec.wave, and the OPD of every ray against n_foc reference spheres per tile
+ * (csrc/rt_refocus.cuh; DESIGN.md section 4): the reference's wave_abr_pre_calc once per ray,
+ * wave_abr_calc once per sphere.  The focus-independent columns of each tile's wave record are used
+ * (finite: 0-16, 22, 23; infinite reference, [21] == 0: 0-12, 17-20, 22, 23).
+ * spheres: DEVICE [n_foc][n_tiles][RT_SPHERE_DOUBLES], what calculate_reference_sphere changes with
+ *   the focus: 0-2 ref_dir  3 ref_sphere_radius  4 sign_soln (+1/-1; 0 on infinite-reference tiles)
+ *   5-7 image_pt.  A plane whose record equals the tile's own (wave 17-21) gives rt_trace_grid's opd
+ *   bit for bit on finite tiles; infinite-reference tiles round as the reference's focus_wavefront.
+ * 1 <= n_foc <= RT_MAX_FOCUS.  opd_planes: DEVICE [n_foc][n] with n the rays of the range: entry
+ *   k*n + r is plane k's OPD (system units) of ray r of the range, indexed as rt_trace_grid's
+ *   outputs; NaN on every plane for rays with status != 0.
+ * out: per-ray results of kind 0 (p, d, op, status, fail_surf, n_seg); opd, abr_x, abr_y and full
+ *   must be NULL.  opd_planes may be NULL for an empty range.  RT_ERR_INVALID for bad arguments and RT_ERR_UNSUPPORTED where rt_trace_grid's opd
+ *   is unsupported, both before any device work.  One launch on `stream` (none for an empty range). */
+int rt_trace_grid_opd_focus(const rt_table *table, const rt_grid *grid,
+                            int64_t chunk_begin, int64_t chunk_end, const rt_opts *opts,
+                            const double *spheres, int32_t n_foc,
+                            const rt_out *out, double *opd_planes, void *stream);
 
 /* ---- misc */
 const char *rt_last_error(void);

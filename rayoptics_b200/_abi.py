@@ -22,6 +22,7 @@ RT_ZERN_DOUBLES = 752
 RT_ZERN_MAX_TERMS = 37
 RT_MTF_MAX_RAYS = 1024
 RT_MTF_DOUBLES = 8
+RT_SPHERE_DOUBLES = 8
 
 # enum rt_profile
 PROFILE_IDS = {'Spherical': 0, 'Conic': 1, 'EvenPolynomial': 2,
@@ -127,7 +128,7 @@ EXPORTS = ['rt_table_create', 'rt_table_destroy', 'rt_table_dims', 'rt_table_set
            'rt_selftest_division', 'rt_grid_chief_ref_focus', 'rt_grid_focus_scratch_bytes',
            'rt_trace_grid_focus', 'rt_grid_wfe_scratch_bytes', 'rt_trace_grid_wfe', 'rt_combine_wfe',
            'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike', 'rt_grid_aim_chief',
-           'rt_grid_pupil_function', 'rt_grid_mtf']
+           'rt_grid_pupil_function', 'rt_grid_mtf', 'rt_grid_mtf_shifts', 'rt_trace_grid_opd_focus']
 
 _lib = None
 
@@ -207,6 +208,10 @@ def load_library():
     lib.rt_grid_pupil_function.restype = i32
     lib.rt_grid_mtf.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     lib.rt_grid_mtf.restype = i32
+    lib.rt_grid_mtf_shifts.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp, vp, vp]
+    lib.rt_grid_mtf_shifts.restype = i32
+    lib.rt_trace_grid_opd_focus.argtypes = [vp, vp, i64, i64, C.POINTER(rt_opts), vp, i32, C.POINTER(rt_out), vp, vp]
+    lib.rt_trace_grid_opd_focus.restype = i32
     lib.rt_last_error.restype = C.c_char_p
     lib.rt_abi_version.restype = i32
     lib.rt_chunk_rays.restype = i32

@@ -369,10 +369,15 @@ def wavefront_grid_args(opt_model, table, num_rays, fields, wvls, foc, image_pt_
     and reference spheres of all tiles (one ``waveabr.setup_tiles`` call), each field's ``RayGrid``
     pupil samples, no vignetting applied.  ``ref_wvl_for_image_pt``: refer every wavelength to that
     wavelength's chief-ray image point (``setup_tiles``); by default each its own"""
-    sm = opt_model.seq_model
     wave, ref_img, _ = W.setup_tiles(opt_model, table, fields, wvls, foc, image_pt_2d, image_delta,
                                      ref_wvl_for_image_pt=ref_wvl_for_image_pt,
                                      chief_tracer=None if backend is None else backend.chief_rays)
+    return _wavefront_grid_args(opt_model, table, num_rays, fields, wvls, foc, wave, ref_img)
+
+
+def _wavefront_grid_args(opt_model, table, num_rays, fields, wvls, foc, wave, ref_img):
+    """the PupilGrid arguments of wavefront_grid_args for given tile records"""
+    sm = opt_model.seq_model
     pupils = [_wavefront_pupil(opt_model, fld, num_rays) for fld in fields]
     recs, eprad, z_pupil = grid_fields_of(opt_model, fields)
     wvl_idx = [sm.index_for_wavelength(w) if table is None else table.wvl_index(w) for w in wvls]
@@ -683,6 +688,190 @@ def mtf(opt_model, num_rays=64, fields=None, wvls=None, foc=None, image_pt_2d=No
             out['poly_x'] = polychromatic_mtf(out['otf_x_at'], wts)
             out['poly_y'] = polychromatic_mtf(out['otf_y_at'], wts)
     return MTF(**out)
+
+
+class ThroughFocusWavefront:
+    """Result of ``through_focus_wavefront``; plane k is focus shift ``foc[k]``.
+
+    ``coef`` ``[K, n_fields, n_wvls, num_terms]``: Fringe Zernike coefficients in waves; ``rms``, ``pv``
+    ``[K, n_fields, n_wvls]`` (piston removed, waves) and ``rms_wfe``: the RMS with piston and tilt
+    removed (the 3-term fit's residual); ``strehl``: |sum P|^2/n_used^2 at plane k's reference point;
+    ``ref_img`` ``[K, n_fields, n_wvls, 2]``; ``n_used`` and the ray counts ``n_ok``, ``n_missed``,
+    ``n_tir``, ``n_blocked``, ``n_other`` ``[n_fields, n_wvls]`` (status does not depend on the focus);
+    ``best_index_strehl`` / ``best_foc_strehl`` and ``best_index_rms`` / ``best_foc_rms`` ``[n_fields,
+    n_wvls]``: the sampled plane of greatest Strehl ratio and of least ``rms_wfe`` (-1 / NaN where no
+    ray is used).  With ``freqs`` ``[F]``: ``otf_x_at``, ``otf_y_at``, ``mtf_x_at``, ``mtf_y_at`` ``[K,
+    n_fields, n_wvls, F]``, ``cutoff`` ``[K, n_fields, n_wvls]`` and ``shifts``, the pupil shifts whose
+    autocorrelation was summed; polychromatic: ``poly_x``, ``poly_y`` ``[K, n_fields, F]`` and ``wts``.
+    ``zernike_record``, ``mtf_record`` ``[K, n_tiles, ...]``, ``acf_x``, ``acf_y`` ``[K, n_tiles,
+    len(shifts)]``: the raw device records."""
+
+    def __init__(self, **kw):
+        for k, v in kw.items():
+            setattr(self, k, v)
+
+
+def otf_shift_set(freqs, freq):
+    """The native shifts ``otf_at`` reads to interpolate at ``freqs``: 0 and, for every tile (row of
+    ``freq`` ``[..., N]`` with finite frequencies) and frequency, the two shifts of the bracket that
+    ``np.interp`` finds in that row, widened by one on each side.  ``otf_at`` on the rows restricted to
+    these shifts gives the same bits as on all N: the bracket, its slope and the end rules (the value
+    at the last shift, 0 past it) are the same.  Sorted, unique, int."""
+    freq = np.asarray(freq, dtype=np.float64)
+    n = freq.shape[-1]
+    rows = freq.reshape(-1, n)
+    keep = {0}
+    for row in rows[np.isfinite(rows).all(axis=1)]:
+        j = np.searchsorted(row, np.asarray(freqs, dtype=np.float64), side='right') - 1
+        for d in (-1, 0, 1, 2):
+            keep.update(np.clip(j + d, 0, n - 1).tolist())
+    return np.array(sorted(keep), dtype=np.int64)
+
+
+def _opd_planes_host(opt_model, spec, fields, wvls, foc, full, op, status, pkgs):
+    """``[K, n_rays]`` OPD of traced whole rays against every plane's reference sphere: the
+    reference's rapid refocus, ``waveabr.wave_abr_pre_calc`` once per ray and ``wave_abr_calc`` per
+    plane (the ``backend=`` seam of ``through_focus_wavefront``)"""
+    fod = opt_model['analysis_results']['parax_data'].fod
+    per, n_ifc = spec.rays_per_tile, full.shape[0]
+    out = np.full((len(foc), spec.n_rays), np.nan)
+    for t in range(spec.n_tiles):
+        fi, wi = divmod(t, spec.n_wvls)
+        fld, wvl = fields[fi], wvls[wi]
+        crp, rs0 = pkgs[0][fi][wi]
+        for r in range(t*per, (t + 1)*per):
+            if status[r] != 0:
+                continue
+            ray = [[full[k, 0:3, r], full[k, 3:6, r], float(full[k, 6, r]), full[k, 7:10, r]] for k in range(n_ifc)]
+            ray_pkg = (ray, float(op[r]), wvl)
+            pre = W.wave_abr_pre_calc(fod, fld, wvl, foc[0], ray_pkg, crp, rs0)
+            for k in range(len(foc)):
+                out[k, r] = W.wave_abr_calc(fod, fld, wvl, foc[k], ray_pkg, crp, pre, pkgs[k][fi][wi][1])
+    return out
+
+
+def through_focus_wavefront(opt_model, num_rays=64, foc=None, num_planes=21, num_terms=9, freqs=None,
+                            polychromatic=False, fields=None, wvls=None, image_pt_2d=None, image_delta=None,
+                            table=None, device=0, backend=None, **trace_kwargs):
+    """Zernike terms, RMS wavefront error, Strehl ratio and (with ``freqs``) the MTF of every field and
+    wavelength at every focus shift of ``foc``, from one grid trace.
+
+    The rays are those of ``zernike_fit`` and ``mtf`` (``RayGrid``'s ``num_rays`` x ``num_rays`` samples,
+    no vignetting applied, apertures checked; a ray is used when its status is 0 and x^2 + y^2 <= 1).
+    ``foc``: absolute focus shifts, as ``through_focus`` (default ``focus_planes(osp.defocus,
+    num_planes)``), 1 ... RT_MAX_FOCUS of them.  The chief rays are traced once and give every plane's
+    reference sphere (``waveabr.setup_tiles_focus``); one ``rt_trace_grid_opd_focus`` launch traces the
+    grid and evaluates each ray's OPD against every sphere; then per plane ``rt_grid_zernike``
+    (``num_terms``: 3 ... 37, default 9, through primary spherical), ``rt_grid_pupil_function`` and
+    ``rt_grid_mtf_shifts`` at the pupil shifts that ``otf_at`` reads for ``freqs`` (none without them:
+    the Strehl ratio needs the record only).  On finite-reference tiles plane k equals
+    ``zernike_fit(foc=foc[k])`` and ``mtf(foc=foc[k])`` bit for bit; tiles with an infinite reference
+    sphere round as the reference's ``focus_wavefront``.  ``polychromatic``: refer every wavelength to
+    the central wavelength's chief-ray image point, as ``mtf``.  ``backend``: the CPU test seam (the
+    reference's ``wave_abr_pre_calc`` / ``wave_abr_calc`` on traced whole rays).  ``trace_kwargs``:
+    trace options.  Returns a ``ThroughFocusWavefront``."""
+    n = int(num_rays)
+    if not 1 <= n <= E.RT_MTF_MAX_RAYS:
+        raise ValueError(f'num_rays must be 1 ... {E.RT_MTF_MAX_RAYS}')
+    if not 3 <= int(num_terms) <= E.RT_ZERN_MAX_TERMS:
+        raise ValueError(f'num_terms must be 3 ... {E.RT_ZERN_MAX_TERMS}')
+    num_terms = int(num_terms)
+    if polychromatic and freqs is None:
+        raise ValueError('polychromatic=True needs freqs=')
+    if freqs is not None:
+        freqs = np.asarray(freqs, dtype=np.float64).reshape(-1)
+        if not (np.isfinite(freqs).all() and (freqs >= 0).all()):
+            raise ValueError('freqs must be finite and >= 0')
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    foc = focus_planes(osp.defocus, num_planes) if foc is None else E._focus_array(foc)
+    if not (1 <= len(foc) <= E._abi.RT_MAX_FOCUS and np.isfinite(foc).all()):
+        raise ValueError(f'foc must hold 1 ... {E._abi.RT_MAX_FOCUS} finite focus shifts')
+    fields = list(osp.field_of_view.fields if fields is None else fields)
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    ref_wvl = None
+    if polychromatic:
+        ref_wvl = sm.central_wavelength()
+        if ref_wvl not in wvls:
+            raise ValueError('polychromatic=True needs the central wavelength among wvls')
+    K, nf, nw = len(foc), len(fields), len(wvls)
+    nt = nf*nw
+    tab = None if backend is not None else _table_for(opt_model, table, device)
+    wave, ref_img, spheres, pkgs = W.setup_tiles_focus(
+        opt_model, tab, fields, wvls, foc, image_pt_2d, image_delta, ref_wvl_for_image_pt=ref_wvl,
+        chief_tracer=None if backend is None else backend.chief_rays)
+    args, grid_kw = _wavefront_grid_args(opt_model, tab, n, fields, wvls, foc[0], wave[0], ref_img[0])
+    lam = np.array([[opt_model.nm_to_sys_units(w) for w in wvls]]*nf).ravel()
+    fod = opt_model['analysis_results']['parax_data'].fod
+    fx, cut, fy = zip(*[mtf_frequencies(args[2], wave[k], lam, fod.exp_radius)
+                        + mtf_frequencies(args[3], wave[k], lam, fod.exp_radius)[:1] for k in range(K)])
+    shifts = (np.zeros(0, dtype=np.int64) if freqs is None
+              else otf_shift_set(freqs, np.concatenate([np.array(fx), np.array(fy)])))
+    m = len(shifts)
+    trace_kwargs.setdefault('check_apertures', True)
+    if backend is not None:
+        spec = E.PupilGridSpec(*args, **grid_kw)
+        full, op, status = backend.trace_rays(opt_model, spec, trace_kwargs['check_apertures'])
+        planes = _opd_planes_host(opt_model, spec, fields, wvls, foc, full, op, status, pkgs)
+        zrec, acf_x, acf_y, mrec = [], [], [], []
+        for k in range(K):
+            zrec.append(_zernike_sums_host(spec, status, planes[k], num_terms))
+            cx, cy, r = _mtf_host(spec, status, planes[k], lam)
+            acf_x.append(cx[:, shifts])
+            acf_y.append(cy[:, shifts])
+            mrec.append(r)
+        zrec, acf_x, acf_y, mrec = (np.array(v) for v in (zrec, acf_x, acf_y, mrec))
+    else:
+        dev = torch.device('cuda', tab.device)
+        with torch.cuda.device(dev):
+            grid = E.PupilGrid(*args, device=tab.device, **grid_kw)
+            planes, res = E.trace_grid_opd_focus(tab, grid, spheres.reshape(K, nt, -1), **trace_kwargs)
+            parts, pup = [], None
+            sh_d = torch.as_tensor(shifts.astype(np.int32), device=dev)      # one upload for every plane
+            for k in range(K):
+                z = E.grid_zernike(grid, 0, grid.n_chunks, num_terms, res.status, planes[k])
+                pup = E.grid_pupil_function(grid, res.status, planes[k], lam, out=pup)
+                cx, cy, r = E.grid_mtf_shifts(grid, res.status, pup[0], pup[1], sh_d)
+                parts += [z.reshape(-1), torch.view_as_real(cx).reshape(-1), torch.view_as_real(cy).reshape(-1),
+                          r.reshape(-1)]
+            host = torch.cat(parts).cpu().numpy()                  # one small copy; waits
+            grid.close()
+        sizes = (nt*E.RT_ZERN_DOUBLES, nt*m*2, nt*m*2, nt*E.RT_MTF_DOUBLES)
+        per_plane = np.split(host, np.cumsum(sizes*K)[:-1])
+        zrec = np.array(per_plane[0::4]).reshape(K, nt, E.RT_ZERN_DOUBLES)
+        acf_x = np.array(per_plane[1::4]).view(np.complex128).reshape(K, nt, m)
+        acf_y = np.array(per_plane[2::4]).view(np.complex128).reshape(K, nt, m)
+        mrec = np.array(per_plane[3::4]).reshape(K, nt, E.RT_MTF_DOUBLES)
+    lam_k = np.tile(lam, K)
+    zs = E.zernike_statistics(zrec.reshape(K*nt, -1), lam_k, num_terms)
+    z3 = E.zernike_statistics(zrec.reshape(K*nt, -1), lam_k, 3)
+    shape = (K, nf, nw)
+    with np.errstate(invalid='ignore', divide='ignore'):
+        strehl = ((mrec[..., 6]**2 + mrec[..., 7]**2)/mrec[..., 5]**2).reshape(shape)
+    rms_wfe = z3['rms_residual'].reshape(shape)
+    n_used = zs['n_used'].reshape(shape)
+    out = dict(foc=foc, coef=zs['coef'].reshape(shape + (num_terms,)), rms=zs['rms'].reshape(shape),
+               pv=zs['pv'].reshape(shape), rms_wfe=rms_wfe, strehl=strehl, ref_img=ref_img,
+               num_rays=n, num_terms=num_terms, n_fields=nf, n_wvls=nw, freqs=freqs, shifts=shifts,
+               polychromatic=bool(polychromatic), zernike_record=zrec, mtf_record=mrec, acf_x=acf_x, acf_y=acf_y)
+    for k in E.ZERN_STATISTICS[:6]:                   # the counts: status does not depend on the focus
+        out[k] = zs[k].reshape(shape)[0]
+    out['best_index_strehl'], out['best_foc_strehl'] = best_focus(foc, -strehl, n_used)
+    out['best_index_rms'], out['best_foc_rms'] = best_focus(foc, rms_wfe, n_used)
+    if freqs is not None:
+        out['cutoff'] = np.array(cut).reshape(shape)
+        for ax, acf, fq in (('x', acf_x, fx), ('y', acf_y, fy)):
+            with np.errstate(invalid='ignore', divide='ignore'):
+                otf = acf/acf[..., :1].real                # shift 0 leads the list: C(0) is real
+            at = np.array([otf_at(freqs, fq[k][:, shifts], otf[k], cut[k]) for k in range(K)])
+            out[f'otf_{ax}_at'] = at.reshape(shape + (-1,))
+            out[f'mtf_{ax}_at'] = np.abs(out[f'otf_{ax}_at'])
+        if polychromatic:
+            region = osp.spectral_region
+            wts = np.array([region.spectral_wts[list(region.wavelengths).index(w)] for w in wvls])
+            out['wts'] = wts
+            out['poly_x'] = np.array([polychromatic_mtf(out['otf_x_at'][k], wts) for k in range(K)])
+            out['poly_y'] = np.array([polychromatic_mtf(out['otf_y_at'][k], wts) for k in range(K)])
+    return ThroughFocusWavefront(**out)
 
 
 class FieldMap:

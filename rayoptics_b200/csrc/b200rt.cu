@@ -16,7 +16,10 @@
  *   k_aim_chief                 chief-ray aiming: the Newton iteration of rt_aim.cuh, one thread
  *                               per field
  *   k_pupil_function, k_mtf     pupil function of a grid trace's per-ray opd / status, and its
- *                               autocorrelation along both pupil axes (rt_mtf.cuh)
+ *                               autocorrelation along both pupil axes, at every or at listed
+ *                               shifts (rt_mtf.cuh)
+ *   k_trace_grid[_lean]_opd_focus  one trace, the OPD of every ray against up to RT_MAX_FOCUS
+ *                               reference spheres (rt_refocus.cuh)
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
  * The surface table (n_ifc x rt_surface_desc + n_wvl x n_ifc indices) is staged
@@ -40,6 +43,7 @@
 #include "rt_zernike.cuh"
 #include "rt_aim.cuh"
 #include "rt_mtf.cuh"
+#include "rt_refocus.cuh"
 
 using namespace b200rt;
 
@@ -502,18 +506,31 @@ __device__ __forceinline__ void wfe_item(bool have, int status, double W, double
     dst[col] = v;
 }
 
+/* ---- OPD at many reference spheres (rt_trace_grid_opd_focus): per ray, refocus_pre once and
+ * refocus_opd per plane (rt_refocus.cuh), after the trace and outside its interface loop */
+struct RefocusPlanes {
+    const double *spheres;      /* DEVICE [n][n_tiles][RT_SPHERE_DOUBLES] */
+    double *planes;             /* DEVICE [n][n_rays]: plane pl of ray k of the range at pl*n_rays + k */
+    int64_t n_rays, sphere_stride;     /* rays of the range; n_tiles*RT_SPHERE_DOUBLES */
+    int32_t n, pad_;
+};
+
 /* chunk loop shared by the general and the lean grid kernels: start ray ->
  * trace -> per-ray results -> transverse aberration (focus_pupil_coords,
  * analyses.py:561-580) -> spot sums.  FOCUS: the spot sums of the planes of *FP instead
  * (needs SUMMARY == false and a work counter).  WFE: the wavefront-error sums of wfe_item instead
- * (needs WAVE, SUMMARY == false and a work counter).  NRML: see store_result. */
-template <bool SUMMARY, bool WAVE, bool FOCUS = false, bool NRML = true, bool WFE = false, typename TraceFn>
+ * (needs WAVE, SUMMARY == false and a work counter).  OPDF: the OPD against every sphere of *RP
+ * instead of out.opd (needs WAVE alone).  NRML: see store_result. */
+template <bool SUMMARY, bool WAVE, bool FOCUS = false, bool NRML = true, bool WFE = false, bool OPDF = false,
+          typename TraceFn>
 __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_begin, int64_t chunk_end,
                                                 const rt_out &out, double *scratch, double *acc,
                                                 unsigned long long *work_counter, double *item_sums,
-                                                TraceFn trace, const FocusPlanes *FP = nullptr)
+                                                TraceFn trace, const FocusPlanes *FP = nullptr,
+                                                const RefocusPlanes *RP = nullptr)
 {
     static_assert(!WFE || (WAVE && !SUMMARY && !FOCUS), "WFE needs the OPD epilogue and no spot sums");
+    static_assert(!OPDF || (WAVE && !SUMMARY && !FOCUS && !WFE), "OPDF needs the OPD epilogue alone");
     const int64_t tile0 = chunk_begin/G.chunks_per_tile;
     const int64_t ray0 = tile0*G.rays_per_tile + (chunk_begin - tile0*G.chunks_per_tile)*RT_BLOCK;
     const int64_t sl = G.chunks_per_tile < RT_MAX_GRID ? G.chunks_per_tile : RT_MAX_GRID;
@@ -564,7 +581,18 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             store_result<NRML>(out, k, R);
             status = R.status; op = R.op;
             if (FOCUS) { fp = R.p; fd = R.d; }
-            if (WAVE) {
+            if (OPDF) {
+                /* every plane of the ray: the sphere records of a work item's tile are warp-uniform loads */
+                double *dst = RP->planes + k;
+                if (R.status == RT_RAY_OK) {
+                    const RefocusRay q = refocus_pre(G.wave + tile*RT_WAVE_DOUBLES, R.p1, d0, R.pk, R.dk, R.p, R.d, R.op);
+                    const double *S = RP->spheres + tile*RT_SPHERE_DOUBLES;
+                    for (int pl = 0; pl < RP->n; pl++)
+                        dst[pl*RP->n_rays] = refocus_opd(q, S + pl*RP->sphere_stride);
+                } else {
+                    for (int pl = 0; pl < RP->n; pl++) dst[pl*RP->n_rays] = CUDART_NAN;
+                }
+            } else if (WAVE) {
                 const double opd = (R.status == RT_RAY_OK)
                                        ? wave_opd(G.wave + tile*RT_WAVE_DOUBLES, R.p1, d0, R.pk, R.dk, R.p, R.d, R.op)
                                        : CUDART_NAN;
@@ -688,6 +716,29 @@ k_trace_grid_wfe(const rt_surface_desc *__restrict__ g_surfs, const double *__re
         });
 }
 
+/* OPD-at-many-spheres instance of k_trace_grid (per-ray outputs of kind 0) */
+template <bool STAGE>
+__global__ void __launch_bounds__(RT_BLOCK)
+k_trace_grid_opd_focus(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                       int n_ifc, int n_wvl, GridDev G, int64_t chunk_begin, int64_t chunk_end,
+                       rt_opts o, rt_out out, const double *__restrict__ g_wvl, int pupil_kind,
+                       unsigned long long *work_counter, RefocusPlanes P)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    const rt_surface_desc *tab;
+    const double *ntab;
+    stage_table<STAGE>(g_surfs, g_n, n_ifc, n_wvl, smem, tab, ntab);
+    grid_chunk_loop<false, true, false, true, false, true>(G, chunk_begin, chunk_end, out, nullptr, nullptr,
+                                                           work_counter, nullptr,
+        [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0) {
+            Vec3 p0;
+            grid_start_ray<false>(G, pupil_kind, f, loc, p0, d0);
+            FullWriter fw = {nullptr, 0};
+            const int wi = G.wvl_idx[w];
+            trace_ray<false, true>(tab, ntab + (int64_t)wi*n_ifc, g_wvl[wi], n_ifc, o, p0, d0, fw, R);
+        }, nullptr, &P);
+}
+
 /* ---- lean kernels: plan built in shared memory by the CTA (rt_lean.cuh) */
 template <int OUT, bool POLY>
 __global__ void __launch_bounds__(RT_BLOCK, POLY ? 2 : RT_LEAN_MIN_CTAS)
@@ -792,6 +843,30 @@ k_trace_grid_lean_wfe(const rt_surface_desc *__restrict__ g_surfs, const double 
             FullWriter fw = {nullptr, 0};
             trace_ray_lean<0, true, POLY>(ls, li + (int64_t)G.wvl_idx[w]*n_ifc, lp, g_surfs, n_ifc, o, p0, d0, fw, R);
         });
+}
+
+/* OPD-at-many-spheres instance of k_trace_grid_lean (per-ray outputs of kind 0) */
+template <bool POLY>
+__global__ void __launch_bounds__(RT_BLOCK, POLY ? 2 : RT_LEAN_MIN_CTAS)
+k_trace_grid_lean_opd_focus(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                            int n_ifc, int n_wvl, GridDev G, int64_t chunk_begin, int64_t chunk_end,
+                            rt_opts o, rt_out out, unsigned long long *work_counter, RefocusPlanes P)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    LeanSurf *ls = reinterpret_cast<LeanSurf *>(smem);
+    LeanIdx *li = reinterpret_cast<LeanIdx *>(ls + n_ifc);
+    LeanPoly *lp = reinterpret_cast<LeanPoly *>(li + (size_t)n_ifc*n_wvl);      /* POLY instances only */
+    build_plan(g_surfs, g_n, n_ifc, n_wvl, o, ls, li);
+    if (POLY) build_poly_plan(g_surfs, n_ifc, lp);
+    __syncthreads();
+    grid_chunk_loop<false, true, false, false, false, true>(G, chunk_begin, chunk_end, out, nullptr, nullptr,
+                                                            work_counter, nullptr,
+        [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0) {
+            Vec3 p0;
+            grid_start_ray<true>(G, RT_PUPIL_EPD, f, loc, p0, d0);
+            FullWriter fw = {nullptr, 0};
+            trace_ray_lean<0, true, POLY>(ls, li + (int64_t)G.wvl_idx[w]*n_ifc, lp, g_surfs, n_ifc, o, p0, d0, fw, R);
+        }, nullptr, &P);
 }
 
 /* division self-test: div_shared/normalize3_shared against the IEEE `/` */
@@ -1234,27 +1309,36 @@ k_pupil_function(GridDev G, int64_t n_rays, const int32_t *__restrict__ status, 
     PT[tile*G.rays_per_tile + j*n + i] = p;
 }
 
-/* One CTA per (tile, slot), slot = 0 ... 2n: slot k < n is Cx(k), n + k is Cy(k), 2n the tile's
- * record.  A thread per line (strided over the CTA) adds its line in index order; thread 0 then adds
- * the line sums in line order (rt_mtf.cuh).  Lines along x are the columns of P and lines along y
- * the columns of PT, so a warp's loads are always 32 adjacent values.  No atomics, no scratch. */
+/* One CTA per (tile, slot), slot = 0 ... 2m with m = n_shifts: slot s < m is Cx(shift s), m + s is
+ * Cy(shift s), 2m the tile's record; shift s is shifts[s], or s itself when shifts is NULL (every
+ * shift, rt_grid_mtf).  A thread per line (strided over the CTA) adds its line in index order;
+ * thread 0 then adds the line sums in line order (rt_mtf.cuh).  Lines along x are the columns of P
+ * and lines along y the columns of PT, so a warp's loads are always 32 adjacent values.  No
+ * atomics, no scratch.  A listed shift outside [0, n-1] gives NaN. */
 __global__ void __launch_bounds__(RT_MTF_THREADS)
 k_mtf(GridDev G, const int32_t *__restrict__ status, const MtfC *__restrict__ P, const MtfC *__restrict__ PT,
-      MtfC *__restrict__ acf_x, MtfC *__restrict__ acf_y, double *__restrict__ rec)
+      const int32_t *__restrict__ shifts, int n_shifts, MtfC *__restrict__ acf_x, MtfC *__restrict__ acf_y,
+      double *__restrict__ rec)
 {
     __shared__ MtfC lines[RT_MTF_MAX_RAYS];
     __shared__ int cnt[RT_MTF_THREADS][6];
-    const int n = G.nx;
-    const int64_t tile = blockIdx.x/(2*n + 1);
-    const int slot = (int)(blockIdx.x - tile*(2*n + 1));
+    const int n = G.nx, m = n_shifts;
+    const int64_t tile = blockIdx.x/(2*m + 1);
+    const int slot = (int)(blockIdx.x - tile*(2*m + 1));
     const int64_t base = tile*G.rays_per_tile;
-    if (slot < 2*n) {
-        const bool ax = slot < n;
-        const int k = ax ? slot : slot - n;
+    if (slot < 2*m) {
+        const bool ax = slot < m;
+        const int s = ax ? slot : slot - m;
+        const int k = shifts ? shifts[s] : s;
+        MtfC *dst = (ax ? acf_x : acf_y) + tile*m + s;
+        if (k < 0 || k >= n) {
+            if (threadIdx.x == 0) *dst = MtfC{CUDART_NAN, CUDART_NAN};
+            return;
+        }
         const MtfC *src = (ax ? P : PT) + base;
         for (int l = threadIdx.x; l < n; l += blockDim.x) lines[l] = mtf_line_shift(src + l, n, n, k);
         __syncthreads();
-        if (threadIdx.x == 0) (ax ? acf_x : acf_y)[tile*n + k] = mtf_line_sum(lines, 1, n);
+        if (threadIdx.x == 0) *dst = mtf_line_sum(lines, 1, n);
         return;
     }
     /* the record: S = sum P (lines along x), the status classes and the used rays */
@@ -2169,6 +2253,65 @@ int rt_trace_grid_focus(const rt_table *t, const rt_grid *g, int64_t chunk_begin
     return RT_OK;
 }
 
+/* the OPD of every ray against n_foc reference spheres (rt_refocus.cuh), one launch in the kernel
+ * family rt_trace_grid takes for an opd launch; the schedule is rt_trace_grid's */
+int rt_trace_grid_opd_focus(const rt_table *t, const rt_grid *g, int64_t chunk_begin, int64_t chunk_end,
+                            const rt_opts *o, const double *spheres, int32_t n_foc, const rt_out *out,
+                            double *opd_planes, void *stream)
+{
+    if (n_foc < 1 || n_foc > RT_MAX_FOCUS)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_opd_focus: n_foc must be in [1, RT_MAX_FOCUS]");
+    if (!t || !g || !out || !spheres || (chunk_end > chunk_begin && !opd_planes))
+        return fail(RT_ERR_INVALID, "rt_trace_grid_opd_focus: table, grid, out, spheres and opd_planes are required");
+    if (out->opd || out->abr_x || out->abr_y || out->full)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_opd_focus: opd, abr_x, abr_y and full must be NULL");
+    if (out_kind(out) != 0)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_opd_focus: normals and dst are not written");
+    if (!g->d_wave)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_opd_focus: the grid has no wave records (rt_grid_spec.wave)");
+    if (t->device != g->device)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_opd_focus: table and grid on different devices");
+    if (chunk_begin < 0 || chunk_end > g->n_chunks || chunk_end < chunk_begin)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_opd_focus: chunk range out of bounds");
+    int rc = check_opts(t, o);
+    if (rc) return rc;
+    for (int32_t wi : g->h_wvl_idx)
+        if (wi < 0 || wi >= t->n_wvl)
+            return fail(RT_ERR_INVALID, "rt_trace_grid_opd_focus: the grid's wvl_idx is out of range for this table");
+    if (!t->wave_ok)
+        return fail(RT_ERR_UNSUPPORTED, "rt_trace_grid_opd_focus: opd needs >= 3 interfaces and no decenter on the last one before the image");
+    if (chunk_begin == chunk_end) return RT_OK;
+    DeviceGuard guard(t->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    RefocusPlanes P;
+    P.spheres = spheres; P.planes = opd_planes;
+    P.n_rays = first_ray_of_chunk(g, chunk_end) - first_ray_of_chunk(g, chunk_begin);
+    P.sphere_stride = g->n_tiles*RT_SPHERE_DOUBLES;
+    P.n = n_foc; P.pad_ = 0;
+    const GridDev G = grid_dev(g);
+    unsigned long long *wc;
+    if ((rc = launch_counter(t, s, &wc))) return rc;
+    int grid;
+    /* angular pupil specifications are generated by the general kernels only (rt_grid.cuh) */
+    if (t->lean && g->pupil_kind == RT_PUPIL_EPD) {
+        auto kern = t->lean_poly ? k_trace_grid_lean_opd_focus<true> : k_trace_grid_lean_opd_focus<false>;
+        if ((rc = prep_kernel(kern, t->lean_bytes))) return rc;
+        if ((rc = persistent_grid(kern, t->lean_bytes, t->sm_count, chunk_end - chunk_begin, &grid))) return rc;
+        kern<<<grid, RT_BLOCK, t->lean_bytes, s>>>(t->d_surfs, t->d_n, t->n_ifc, t->n_wvl, G, chunk_begin, chunk_end,
+                                                   *o, *out, wc, P);
+    } else {
+        auto kern = t->stage ? k_trace_grid_opd_focus<true> : k_trace_grid_opd_focus<false>;
+        const size_t smem = t->stage ? t->stage_bytes : 0;
+        if ((rc = prep_kernel(kern, smem))) return rc;
+        if ((rc = persistent_grid(kern, smem, t->sm_count, chunk_end - chunk_begin, &grid))) return rc;
+        kern<<<grid, RT_BLOCK, smem, s>>>(t->d_surfs, t->d_n, t->n_ifc, t->n_wvl, G, chunk_begin, chunk_end, *o, *out,
+                                          t->d_wvl, g->pupil_kind, wc, P);
+    }
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
 int rt_combine_summaries(const double *parts, int32_t n_parts, int64_t n_tiles, double *out, void *stream)
 {
     if (!parts || !out || n_parts < 1 || n_tiles < 0)
@@ -2338,6 +2481,22 @@ static int mtf_check_grid(const rt_grid *g, const char *fn)
     return RT_OK;
 }
 
+/* one k_mtf launch over n_shifts shifts per axis (shifts NULL: 0 ... n_shifts-1) */
+static int launch_mtf(const rt_grid *g, const int32_t *status, const double *pupil, const double *pupil_t,
+                      const int32_t *shifts, int32_t n_shifts, double *acf_x, double *acf_y, double *record,
+                      void *stream)
+{
+    DeviceGuard guard(g->device);
+    const int n = g->nx;
+    const int threads = n >= RT_MTF_THREADS ? RT_MTF_THREADS : (n + 31)/32*32;
+    k_mtf<<<(unsigned)(g->n_tiles*(2*(int64_t)n_shifts + 1)), threads, 0, (cudaStream_t)stream>>>(
+        grid_dev(g), status, (const MtfC *)pupil, (const MtfC *)pupil_t, shifts, n_shifts, (MtfC *)acf_x,
+        (MtfC *)acf_y, record);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
 int rt_grid_pupil_function(const rt_grid *g, const int32_t *status, const double *opd, const double *wvl_sys,
                            double *pupil, double *pupil_t, void *stream)
 {
@@ -2359,14 +2518,22 @@ int rt_grid_mtf(const rt_grid *g, const int32_t *status, const double *pupil, co
     if (const int rc = mtf_check_grid(g, "rt_grid_mtf")) return rc;
     if (!status || !pupil || !pupil_t || !acf_x || !acf_y || !record)
         return fail(RT_ERR_INVALID, "rt_grid_mtf: status, pupil, pupil_t, acf_x, acf_y and record are required");
-    DeviceGuard guard(g->device);
-    const int n = g->nx;
-    const int threads = n >= RT_MTF_THREADS ? RT_MTF_THREADS : (n + 31)/32*32;
-    k_mtf<<<(unsigned)(g->n_tiles*(2*n + 1)), threads, 0, (cudaStream_t)stream>>>(
-        grid_dev(g), status, (const MtfC *)pupil, (const MtfC *)pupil_t, (MtfC *)acf_x, (MtfC *)acf_y, record);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    return RT_OK;
+    return launch_mtf(g, status, pupil, pupil_t, nullptr, g->nx, acf_x, acf_y, record, stream);
+}
+
+int rt_grid_mtf_shifts(const rt_grid *g, const int32_t *status, const double *pupil, const double *pupil_t,
+                       const int32_t *shifts, int32_t n_shifts, double *acf_x, double *acf_y, double *record,
+                       void *stream)
+{
+    if (n_shifts < 0) return fail(RT_ERR_INVALID, "rt_grid_mtf_shifts: n_shifts out of range");
+    if (const int rc = mtf_check_grid(g, "rt_grid_mtf_shifts")) return rc;
+    if (!status || !pupil || !pupil_t || !record)
+        return fail(RT_ERR_INVALID, "rt_grid_mtf_shifts: status, pupil, pupil_t and record are required");
+    if (g->n_tiles*(2*(int64_t)n_shifts + 1) > INT32_MAX)
+        return fail(RT_ERR_INVALID, "rt_grid_mtf_shifts: n_shifts out of range");
+    if (n_shifts > 0 && (!shifts || !acf_x || !acf_y))
+        return fail(RT_ERR_INVALID, "rt_grid_mtf_shifts: shifts, acf_x and acf_y are required when n_shifts > 0");
+    return launch_mtf(g, status, pupil, pupil_t, shifts, n_shifts, acf_x, acf_y, record, stream);
 }
 
 /* fp64 vector-pipe peak, measured with a DFMA chain kernel: the roofline

@@ -20,7 +20,7 @@ import torch
 
 from . import _abi
 from ._abi import (rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES, RT_WFE_DOUBLES,
-                   RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS, RT_MTF_DOUBLES, RT_MTF_MAX_RAYS)
+                   RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS, RT_MTF_DOUBLES, RT_MTF_MAX_RAYS, RT_SPHERE_DOUBLES)
 
 SUMMARY_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other',
                   'sum_x', 'sum_y', 'sum_xx', 'sum_yy', 'sum_xy',
@@ -803,13 +803,14 @@ def _ray_tensor(t, dt, n, name):
         raise ValueError(f'{name} must be a contiguous {dt} CUDA tensor of {n} entries')
 
 
-def grid_pupil_function(grid, status, opd, wvl_sys):
+def grid_pupil_function(grid, status, opd, wvl_sys, out=None):
     """``rt_grid_pupil_function``: ``(pupil, pupil_t)``, ``[n_tiles, n, n]`` complex128 device tensors
     of the pupil function exp(2 pi i opd/wvl_sys) of every tile of a square product PupilGrid without
     vignetting (0 where a ray is not used: status != 0 or x^2 + y^2 > 1), ``pupil_t`` transposed in
     each tile.  ``status`` (int32), ``opd`` (float64, system units): the per-ray device tensors of a
     grid trace over all chunks; ``wvl_sys``: the wavelength in system units, a scalar or one value per
-    tile.  Asynchronous on the current CUDA stream."""
+    tile.  ``out``: an earlier call's ``(pupil, pupil_t)`` to write into.  Asynchronous on the current
+    CUDA stream."""
     lib = _abi.load_library()
     _ray_tensor(status, torch.int32, grid.n_rays, 'status')
     _ray_tensor(opd, torch.float64, grid.n_rays, 'opd')
@@ -817,8 +818,13 @@ def grid_pupil_function(grid, status, opd, wvl_sys):
     lam = np.broadcast_to(np.asarray(wvl_sys, dtype=np.float64).reshape(-1), (grid.n_tiles,))
     lam = torch.tensor(lam, device=device)
     shape = (grid.n_tiles, grid.nx, grid.ny)
-    pupil = torch.empty(shape, dtype=torch.complex128, device=device)
-    pupil_t = torch.empty(shape, dtype=torch.complex128, device=device)
+    if out is None:
+        pupil = torch.empty(shape, dtype=torch.complex128, device=device)
+        pupil_t = torch.empty(shape, dtype=torch.complex128, device=device)
+    else:
+        pupil, pupil_t = out
+        for t, name in ((pupil, 'pupil'), (pupil_t, 'pupil_t')):
+            _ray_tensor(t, torch.complex128, grid.n_rays, name)
     with torch.cuda.device(device):
         _abi.check(lib.rt_grid_pupil_function(grid.handle, _ptr(status), _ptr(opd), _ptr(lam), _ptr(pupil),
                                               _ptr(pupil_t), _stream_ptr(device)))
@@ -861,6 +867,74 @@ def trace_grid_mtf(table, grid, wvl_sys, res=None, **kwargs):
     acf_x, acf_y, rec = grid_mtf(grid, res.status, pupil, pupil_t)
     rec._keep = (rec._keep, res)
     return acf_x, acf_y, rec, pupil
+
+
+def grid_mtf_shifts(grid, status, pupil, pupil_t, shifts):
+    """``rt_grid_mtf_shifts``: ``grid_mtf`` at the listed shifts only -- ``(acf_x, acf_y, record)`` with
+    ``acf_x``, ``acf_y`` ``[n_tiles, len(shifts)]`` complex128, entry m bit for bit ``grid_mtf``'s entry
+    ``shifts[m]``.  ``shifts``: integers in [0, n-1], any order, duplicates allowed; none gives the
+    record alone.  A contiguous int32 CUDA tensor is passed as it is, without the range check (an entry
+    outside [0, n-1] gives NaN).  Asynchronous on the current CUDA stream."""
+    lib = _abi.load_library()
+    _ray_tensor(status, torch.int32, grid.n_rays, 'status')
+    for t, name in ((pupil, 'pupil'), (pupil_t, 'pupil_t')):
+        _ray_tensor(t, torch.complex128, grid.n_rays, name)
+    device = status.device
+    if torch.is_tensor(shifts) and shifts.is_cuda:
+        _ray_tensor(shifts, torch.int32, shifts.numel(), 'shifts')
+        sh_d = shifts
+    else:
+        sh = np.ascontiguousarray(np.asarray(shifts, dtype=np.int64).reshape(-1))
+        if ((sh < 0) | (sh >= grid.nx)).any():
+            raise ValueError(f'shifts must lie in [0, {grid.nx - 1}]')
+        sh_d = torch.tensor(sh.astype(np.int32), device=device)
+    m = sh_d.numel()
+    acf_x = torch.empty((grid.n_tiles, m), dtype=torch.complex128, device=device)
+    acf_y = torch.empty((grid.n_tiles, m), dtype=torch.complex128, device=device)
+    rec = torch.empty((grid.n_tiles, RT_MTF_DOUBLES), dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        _abi.check(lib.rt_grid_mtf_shifts(grid.handle, _ptr(status), _ptr(pupil), _ptr(pupil_t),
+                                          _ptr(sh_d) if m else None, m,
+                                          _ptr(acf_x) if m else None, _ptr(acf_y) if m else None, _ptr(rec),
+                                          _stream_ptr(device)))
+    rec._keep = (status, pupil, pupil_t, sh_d)
+    return acf_x, acf_y, rec
+
+
+def trace_grid_opd_focus(table, grid, spheres, chunk_begin=0, chunk_end=None, res=None, **kwargs):
+    """The OPD of every ray of chunks ``[chunk_begin, chunk_end)`` of a PupilGrid built with ``wave=``
+    records against K reference spheres per tile, from one trace (``rt_trace_grid_opd_focus``).
+    ``spheres``: ``[K, n_tiles, RT_SPHERE_DOUBLES]`` records (``waveabr.setup_tiles_focus``), numpy or
+    a float64 device tensor.  Returns ``(opd_planes, res)``: the ``[K, n]`` float64 device tensor (row k:
+    plane k's OPD in system units, NaN where status != 0) and the BundleResult of the per-ray ``status``
+    (``res``: one to write into, with any kind-0 outputs).  Trace defaults as ``trace_grid``.
+    Asynchronous on the current CUDA stream."""
+    lib = _abi.load_library()
+    device = torch.device('cuda', table.device)
+    if chunk_end is None:
+        chunk_end = grid.n_chunks
+    kwargs.setdefault('check_apertures', True)
+    kwargs.setdefault('first_surf', 1)
+    kwargs.setdefault('last_surf', table.n_ifc - 2)
+    if grid.pupil_kind == _abi.PUPIL_WIDE:
+        kwargs['intersect_obj'] = False
+    opts = _abi.make_opts(**kwargs)
+    n = grid.rays_in_chunks(chunk_begin, chunk_end)
+    if res is None:
+        res = BundleResult(n, table.n_ifc, device, ('status',))
+    elif res.n != n:
+        raise ValueError('res was allocated for a different number of rays')
+    sph = spheres if torch.is_tensor(spheres) else torch.as_tensor(np.ascontiguousarray(spheres, dtype=np.float64))
+    sph = sph.to(device=device, dtype=torch.float64).contiguous()
+    k = sph.shape[0] if sph.dim() == 3 else 0
+    if sph.dim() != 3 or tuple(sph.shape[1:]) != (grid.n_tiles, RT_SPHERE_DOUBLES):
+        raise ValueError(f'spheres must have shape [K, {grid.n_tiles}, {RT_SPHERE_DOUBLES}]')
+    planes = torch.empty((k, n), dtype=torch.float64, device=device)
+    out = res.c_struct()
+    _abi.check(lib.rt_trace_grid_opd_focus(table.handle, grid.handle, chunk_begin, chunk_end, C.byref(opts),
+                                           _ptr(sph), k, C.byref(out), _ptr(planes), _stream_ptr(device)))
+    planes._keep = sph                     # must outlive the asynchronous launch
+    return planes, res
 
 
 def pupil_function_host(status, opd, x, y, wvl_sys):

@@ -21,7 +21,7 @@ import numpy as np
 
 from . import engine as E
 from .opticalspec import grid_fields_of
-from ._abi import RT_WAVE_DOUBLES
+from ._abi import RT_WAVE_DOUBLES, RT_SPHERE_DOUBLES
 
 
 def normalize(v):
@@ -140,11 +140,57 @@ def setup_tiles(opt_model, table, fields, wvls, foc, image_pt_2d=None, image_del
     ``pkgs[f][w] = (chief_ray_pkg, ref_sphere)``.  ``ref_wvl_for_image_pt``: use
     the image point of that wavelength's chief ray for every wavelength (what
     ``SequentialModel.trace_fan/trace_grid`` do, seq/sequential.py:1015-1040)."""
+    full, op, status = _chief_rays(opt_model, table, fields, wvls, chief_tracer)
+    return _tiles_at(opt_model, full, op, fields, wvls, foc, image_pt_2d, image_delta, ref_wvl_for_image_pt)
+
+
+def setup_tiles_focus(opt_model, table, fields, wvls, focs, image_pt_2d=None, image_delta=None,
+                      ref_wvl_for_image_pt=None, chief_tracer=None):
+    """``setup_tiles`` at every focus shift of ``focs`` from one chief-ray trace.
+
+    Returns ``(wave [K, n_f, n_w, 24], ref_img [K, n_f, n_w, 2], spheres [K, n_f, n_w,
+    RT_SPHERE_DOUBLES], pkgs)``: plane k's ``wave``, ``ref_img`` and ``pkgs[k]`` are
+    ``setup_tiles(..., foc=focs[k])``'s, and its sphere records (``sphere_record``) the part of them
+    that depends on the focus.  A tile
+    whose reference sphere is finite at one plane and infinite at another raises ValueError."""
+    full, op, status = _chief_rays(opt_model, table, fields, wvls, chief_tracer)
+    waves, refs, spheres, all_pkgs = [], [], [], []
+    for foc in focs:
+        wave, ref_img, pkgs = _tiles_at(opt_model, full, op, fields, wvls, foc, image_pt_2d, image_delta,
+                                        ref_wvl_for_image_pt)
+        waves.append(wave)
+        refs.append(ref_img)
+        all_pkgs.append(pkgs)
+        spheres.append([[sphere_record(wave[fi, wi], rs) for wi, (_, rs) in enumerate(row)]
+                        for fi, row in enumerate(pkgs)])
+    wave = np.array(waves)
+    inf = wave[..., 21] == 0.0
+    if (inf != inf[:1]).any():
+        raise ValueError('a tile\'s reference sphere is finite at some focus shifts and infinite at others')
+    return wave, np.array(refs), np.array(spheres), all_pkgs
+
+
+def sphere_record(W, ref_sphere):
+    """The RT_SPHERE_DOUBLES record of a tile (layout: include/b200rt.h rt_trace_grid_opd_focus) from its
+    wave record ``W`` and ``calculate_reference_sphere``'s result: ref_dir, radius, sign_soln (0 on tiles
+    of the infinite-reference variant), image_pt."""
+    image_pt, ref_dir, radius, _ = ref_sphere
+    S = np.zeros(RT_SPHERE_DOUBLES)
+    S[0:3], S[3], S[4], S[5:8] = ref_dir, radius, W[21], image_pt
+    return S
+
+
+def _chief_rays(opt_model, table, fields, wvls, chief_tracer):
     # chief_tracer: test seam (the CPU suite feeds the oracle), same role as trace.py's tracer=
     full, op, status = (trace_chief_rays(opt_model, table, fields, wvls) if chief_tracer is None
                         else chief_tracer(opt_model, fields, wvls))
     if (status != 0).any():
         raise RuntimeError('a chief ray did not reach the image')
+    return full, op, status
+
+
+def _tiles_at(opt_model, full, op, fields, wvls, foc, image_pt_2d, image_delta, ref_wvl_for_image_pt):
+    """the body of setup_tiles for traced chief rays"""
     nf, nw = len(fields), len(wvls)
     wave = np.zeros((nf, nw, RT_WAVE_DOUBLES))
     ref_img = np.zeros((nf, nw, 2))
