@@ -49,6 +49,7 @@ extern "C" {
 #define RT_MTF_MAX_RAYS 1024 /* pupil samples per side of rt_grid_pupil_function / rt_grid_mtf */
 #define RT_MTF_DOUBLES 8     /* per-tile record of rt_grid_mtf */
 #define RT_SPHERE_DOUBLES 8  /* per-(plane, tile) reference-sphere record of rt_trace_grid_opd_focus */
+#define RT_TOL_DOUBLES 24    /* per-(variant, tile) record of rt_trace_grid_variants */
 
 /* error codes (function return values) */
 enum rt_error {
@@ -213,6 +214,7 @@ typedef struct rt_out {
 
 typedef struct rt_table rt_table;
 typedef struct rt_grid rt_grid;
+typedef struct rt_variants rt_variants;
 
 /* ---- table: the compiled form of SequentialModel.path() for all wavelengths */
 
@@ -504,6 +506,31 @@ int rt_trace_grid_opd_focus(const rt_table *table, const rt_grid *grid,
                             int64_t chunk_begin, int64_t chunk_end, const rt_opts *opts,
                             const double *spheres, int32_t n_foc,
                             const rt_out *out, double *opd_planes, void *stream);
+
+/* ---- tolerance analysis: many perturbed prescriptions of one shape over one grid
+ * rt_variants_create: n_var surface tables in one device allocation and one copy.
+ *   surfs: HOST [n_var][n_ifc]; n_by_wvl: HOST [n_var][n_wvl][n_ifc]; wvl_nm: HOST [n_wvl] in nm, or
+ *   NULL (phase elements then see NaN).  The handle is immutable and has its own work counters. */
+int rt_variants_create(const rt_surface_desc *surfs, int32_t n_ifc, const double *n_by_wvl, int32_t n_wvl,
+                       int32_t n_var, const double *wvl_nm, int32_t device, rt_variants **out);
+int rt_variants_destroy(rt_variants *variants);
+/* bytes of scratch rt_trace_grid_variants needs for n_var variants (proportional to the rays) */
+int64_t rt_grid_variants_scratch_bytes(const rt_grid *grid, int32_t n_var);
+/* The whole grid traced once per variant of [var_begin, var_end) in one persistent launch (the general
+ * kernel, the table read from global memory), then one reduction.  The start rays, the reference image
+ * points and foc are the grid's, shared by every variant; no per-ray data is written.
+ * record: DEVICE [var_end - var_begin][n_tiles][RT_TOL_DOUBLES]:
+ *   0-15  rt_trace_grid's summary layout (counts, sum x, y, xx, yy, xy, min / max x, y, sum op, 0);
+ *         equal to rt_trace_grid's summary of a table of that variant alone (dynamic schedule)
+ *   16-21 sum ux, uy, ux*ux, uy*uy, ax*ux, ay*uy over the status-0 rays: ux = dx/dz, uy = dy/dz of the
+ *         last segment (one IEEE division each), (ax, ay) the transverse aberration
+ *   22-23 zero
+ * Sum order (DESIGN.md section 4): summands rounded once, the work-item halving tree, reduce_tile
+ * over a tile's work items in item order.  RT_ERR_INVALID, before any device work, for a bad variant
+ * range, NULL pointers, variants and grid on different devices, opts.wvl_idx or a grid wvl_idx out of
+ * range.  Two launches on `stream` (none for an empty range). */
+int rt_trace_grid_variants(const rt_variants *variants, const rt_grid *grid, int32_t var_begin, int32_t var_end,
+                           const rt_opts *opts, double *record, void *scratch, void *stream);
 
 /* ---- misc */
 const char *rt_last_error(void);

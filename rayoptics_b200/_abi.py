@@ -23,6 +23,7 @@ RT_ZERN_MAX_TERMS = 37
 RT_MTF_MAX_RAYS = 1024
 RT_MTF_DOUBLES = 8
 RT_SPHERE_DOUBLES = 8
+RT_TOL_DOUBLES = 24
 
 # enum rt_profile
 PROFILE_IDS = {'Spherical': 0, 'Conic': 1, 'EvenPolynomial': 2,
@@ -128,7 +129,8 @@ EXPORTS = ['rt_table_create', 'rt_table_destroy', 'rt_table_dims', 'rt_table_set
            'rt_selftest_division', 'rt_grid_chief_ref_focus', 'rt_grid_focus_scratch_bytes',
            'rt_trace_grid_focus', 'rt_grid_wfe_scratch_bytes', 'rt_trace_grid_wfe', 'rt_combine_wfe',
            'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike', 'rt_grid_aim_chief',
-           'rt_grid_pupil_function', 'rt_grid_mtf', 'rt_grid_mtf_shifts', 'rt_trace_grid_opd_focus']
+           'rt_grid_pupil_function', 'rt_grid_mtf', 'rt_grid_mtf_shifts', 'rt_trace_grid_opd_focus',
+           'rt_variants_create', 'rt_variants_destroy', 'rt_grid_variants_scratch_bytes', 'rt_trace_grid_variants']
 
 _lib = None
 
@@ -212,6 +214,15 @@ def load_library():
     lib.rt_grid_mtf_shifts.restype = i32
     lib.rt_trace_grid_opd_focus.argtypes = [vp, vp, i64, i64, C.POINTER(rt_opts), vp, i32, C.POINTER(rt_out), vp, vp]
     lib.rt_trace_grid_opd_focus.restype = i32
+    lib.rt_variants_create.argtypes = [C.POINTER(rt_surface_desc), i32, c_double_p, i32, i32, c_double_p, i32,
+                                       C.POINTER(vp)]
+    lib.rt_variants_create.restype = i32
+    lib.rt_variants_destroy.argtypes = [vp]
+    lib.rt_variants_destroy.restype = i32
+    lib.rt_grid_variants_scratch_bytes.argtypes = [vp, i32]
+    lib.rt_grid_variants_scratch_bytes.restype = i64
+    lib.rt_trace_grid_variants.argtypes = [vp, vp, i32, i32, C.POINTER(rt_opts), vp, vp, vp]
+    lib.rt_trace_grid_variants.restype = i32
     lib.rt_last_error.restype = C.c_char_p
     lib.rt_abi_version.restype = i32
     lib.rt_chunk_rays.restype = i32

@@ -1534,3 +1534,189 @@ def calc_psf(wavefront, ndim, maxdim, device=0):
     AP = torch.fft.fftshift(torch.fft.fft2(torch.fft.fftshift(phase))).abs()**2
     AP = AP/AP.max()
     return AP.cpu().numpy()
+
+
+# ---------------------------------------------------------------- tolerance analysis
+class TolMerit:
+    """The spot merit of every variant of a tolerance run (``tol_merit``): ``merit`` / ``focus``
+    ``[n_var]`` M(delta*) and delta*; ``merit0`` ``[n_var]`` M(0), at the grid's focus; ``n_ok``
+    ``[n_var, n_fields]`` rays that reach the image (all wavelengths); ``centroid`` ``[n_var,
+    n_fields, 2]`` the polychromatic centroid at delta*, ``centroid_shift`` the same minus variant 0's."""
+
+    def __init__(self, merit, focus, merit0, n_ok, centroid):
+        self.merit, self.focus, self.merit0, self.n_ok, self.centroid = merit, focus, merit0, n_ok, centroid
+        self.centroid_shift = centroid - centroid[:1]
+
+
+def _tol_moments(rec, wvl_wts):
+    """per (variant, field) the spectrally weighted sums N, X1, U1, X2, XU, U2 (and for y) of the
+    records ``[n_var, n_fields, n_wvls, RT_TOL_DOUBLES]``"""
+    w = np.asarray(wvl_wts, dtype=np.float64)[None, None, :, None]
+    s = (rec*w).sum(axis=2)
+    return {'n': s[..., 0], 'x1': s[..., 5], 'y1': s[..., 6], 'x2': s[..., 7], 'y2': s[..., 8],
+            'u1': s[..., 16], 'v1': s[..., 17], 'u2': s[..., 18], 'v2': s[..., 19],
+            'xu': s[..., 20], 'yv': s[..., 21]}
+
+
+def tol_sigma2(m, delta):
+    """sigma_f^2(delta) ``[n_var, n_fields]``: the polychromatic mean square spot radius about the
+    polychromatic centroid at defocus ``delta`` (``[n_var]`` or scalar) from the grid's focus,
+    from the moments of ``_tol_moments``: X1 = x1 + delta u1, X2 = x2 + 2 delta xu + delta^2 u2"""
+    d = np.asarray(delta, dtype=np.float64)
+    d = d[:, None] if d.ndim else d
+    n = m['n']
+    with np.errstate(invalid='ignore', divide='ignore'):
+        X1, Y1 = m['x1'] + d*m['u1'], m['y1'] + d*m['v1']
+        X2 = m['x2'] + 2.0*d*m['xu'] + d*d*m['u2']
+        Y2 = m['y2'] + 2.0*d*m['yv'] + d*d*m['v2']
+        s2 = (X2 + Y2)/n - (X1*X1 + Y1*Y1)/(n*n)
+    return np.where(n > 0, s2, np.nan)
+
+
+def tol_merit(rec, wvl_wts, field_wts, compensate_focus=True):
+    """``TolMerit`` of tolerance records ``[n_var, n_fields, n_wvls, RT_TOL_DOUBLES]``:
+    M(delta) = sqrt(sum_f W_f sigma_f^2(delta) / sum_f W_f), quadratic in delta under the root;
+    delta* = -B / 2A of M^2 = A delta^2 + B delta + C (0 where A <= 0 or not ``compensate_focus``).
+    A field without rays makes its variant's merit NaN."""
+    rec = np.asarray(rec, dtype=np.float64)
+    m = _tol_moments(rec, wvl_wts)
+    W = np.asarray(field_wts, dtype=np.float64)
+    n = m['n']
+    with np.errstate(invalid='ignore', divide='ignore'):
+        a2 = (m['u2'] + m['v2'])/n - (m['u1']*m['u1'] + m['v1']*m['v1'])/(n*n)
+        a1 = 2.0*(m['xu'] + m['yv'])/n - 2.0*(m['x1']*m['u1'] + m['y1']*m['v1'])/(n*n)
+        A = (a2*W).sum(axis=1)/W.sum()
+        B = (a1*W).sum(axis=1)/W.sum()
+        focus = np.where(A > 0, -B/(2.0*A), 0.0) if compensate_focus else np.zeros(len(A))
+    focus = np.where(np.isfinite(focus), focus, 0.0)
+
+    def merit_at(d):
+        return np.sqrt(np.maximum((tol_sigma2(m, d)*W).sum(axis=1)/W.sum(), 0.0))
+
+    with np.errstate(invalid='ignore', divide='ignore'):
+        cen = np.stack([(m['x1'] + focus[:, None]*m['u1'])/n, (m['y1'] + focus[:, None]*m['v1'])/n], axis=-1)
+    return TolMerit(merit_at(focus), focus, merit_at(np.zeros(len(focus))), rec[..., 0].sum(axis=2), cen)
+
+
+class Sensitivity:
+    """Result of ``tolerance_sensitivity``.  ``nominal`` / ``nominal_focus``: M and delta* of the
+    nominal system; per tolerance ``merit_plus`` / ``merit_minus`` (at +-delta), ``delta_plus`` /
+    ``delta_minus`` (their change of M), ``focus_plus`` / ``focus_minus``; ``estimated`` = M0 +
+    sqrt(sum_i max(dM_i+, dM_i-, 0)^2); ``result``: the ``TolMerit`` of every variant (0 nominal,
+    then +delta, -delta per tolerance)."""
+
+    def __init__(self, tolerances, res):
+        self.tolerances, self.result = list(tolerances), res
+        self.nominal, self.nominal_focus = float(res.merit[0]), float(res.focus[0])
+        self.merit_plus, self.merit_minus = res.merit[1::2].copy(), res.merit[2::2].copy()
+        self.focus_plus, self.focus_minus = res.focus[1::2].copy(), res.focus[2::2].copy()
+        self.delta_plus, self.delta_minus = self.merit_plus - self.nominal, self.merit_minus - self.nominal
+        worst = np.maximum(np.maximum(self.delta_plus, self.delta_minus), 0.0)
+        self.estimated = self.nominal + float(np.sqrt(np.sum(worst*worst)))
+
+
+class MonteCarlo:
+    """Result of ``tolerance_monte_carlo``: ``values`` ``[num_trials, n_tol]`` the drawn changes;
+    ``merit`` / ``focus`` ``[num_trials]``; ``nominal``; ``mean``, ``std`` and ``percentiles``
+    {50, 80, 90, 98: M} of the trials' merits; ``result``: the ``TolMerit`` (variant 0 nominal)."""
+
+    def __init__(self, tolerances, values, res):
+        self.tolerances, self.values, self.result = list(tolerances), values, res
+        self.nominal = float(res.merit[0])
+        self.merit, self.focus = res.merit[1:].copy(), res.focus[1:].copy()
+        self.mean, self.std = float(np.mean(self.merit)), float(np.std(self.merit))
+        self.percentiles = {p: float(np.percentile(self.merit, p)) for p in (50, 80, 90, 98)}
+
+
+def draw_tolerances(tolerances, num_trials, seed=0, distribution='normal'):
+    """``[num_trials, n_tol]`` changes, trial-major from ``Generator(PCG64(seed))``: 'normal' with
+    sigma = delta/2, truncated to +-delta by drawing again; 'uniform' on [-delta, delta]"""
+    if distribution not in ('normal', 'uniform'):
+        raise ValueError(f'unknown distribution {distribution!r}')
+    rng = np.random.Generator(np.random.PCG64(seed))
+    out = np.zeros((int(num_trials), len(tolerances)))
+    for t in range(int(num_trials)):
+        for i, tol in enumerate(tolerances):
+            dl = abs(float(tol.delta))
+            if distribution == 'uniform':
+                out[t, i] = rng.uniform(-dl, dl)
+                continue
+            v = rng.normal(0.0, dl/2.0)
+            while abs(v) > dl:
+                v = rng.normal(0.0, dl/2.0)
+            out[t, i] = v
+    return out
+
+
+def _tol_records(opt_model, change_sets, num_rays, fields, wvls, foc, table, device, backend, trace_kwargs):
+    """``[n_var, n_fields, n_wvls, RT_TOL_DOUBLES]`` records of the nominal grid for every change
+    set, and the spectral / field weights"""
+    from . import tolerance as TOL
+    from .table import describe_model
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    fields = list(osp.field_of_view.fields if fields is None else fields)
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    foc = osp.defocus.focus_shift if foc is None else foc
+    region = osp.spectral_region
+    wvl_wts = [region.spectral_wts[list(region.wavelengths).index(w)] for w in wvls]
+    field_wts = [f.wt for f in fields]
+    descs, n_by_wvl, all_wvls = describe_model(sm)
+    var = [TOL.perturbed_descriptors(descs, n_by_wvl, ch, sm) for ch in change_sets]
+    nb = np.stack([v[1] for v in var])
+    args, kw = E._grid_args(opt_model, sm.index_for_wavelength, num_rays, fields, wvls, foc, (-1.0, 1.0), True)
+    cwl = sm.index_for_wavelength(sm.central_wavelength())
+    trace_kwargs.setdefault('check_apertures', True)
+    if backend is not None:
+        spec = E.PupilGridSpec(*args, **kw)
+        ref = backend.chief_ref(descs, n_by_wvl, spec, cwl)
+        spec = E.PupilGridSpec(*args, ref_img=np.repeat(ref[:, None, :], len(wvls), axis=1), **kw)
+        rec = np.asarray(backend.trace_variants([v[0] for v in var], nb, spec))
+    else:
+        tab = _table_for(opt_model, table, device)
+        dev = torch.device('cuda', tab.device)
+        with torch.cuda.device(dev):
+            grid = E.PupilGrid(*args, device=tab.device, **kw)
+            grid.chief_ref(tab, cwl)
+            vs = E.VariantSet([v[0] for v in var], nb, all_wvls, device=tab.device)
+            rec = E.trace_grid_variants(vs, grid, **trace_kwargs).cpu().numpy()     # waits
+            vs.close()
+            grid.close()
+    return rec.reshape(len(change_sets), len(fields), len(wvls), -1), wvl_wts, field_wts
+
+
+def tolerance_sensitivity(opt_model, tolerances, num_rays=32, fields=None, wvls=None, foc=None,
+                          compensate_focus=True, table=None, device=0, backend=None, **trace_kwargs):
+    """Change of the spot merit for each tolerance at +delta and -delta, from one grid trace of all
+    variants (``rt_trace_grid_variants``; variant 0 nominal, then +delta, -delta per tolerance).
+
+    The merit M is the field-weighted RMS over fields of the polychromatic (spectral weights) RMS spot
+    radius about its centroid, on the nominal pupil grid with the nominal aim, referred to the nominal
+    chief rays (DESIGN.md section 4); with ``compensate_focus`` each variant is refocused to the
+    delta* that minimises M, solved in closed form from the device sums (no second trace).  The
+    perturbed systems keep the nominal apertures, vignetting and aim (``tolerance.perturbed_model``).
+    ``backend``: the CPU test seam, ``backend.trace_variants(descs, n_by_wvl, grid_spec)`` returning
+    the records and ``backend.chief_ref(descs, n_by_wvl, grid_spec, wvl_idx)`` the reference points."""
+    from . import tolerance as TOL
+    for t in tolerances:
+        TOL.check(opt_model.seq_model, t)
+    sets = [[]]
+    for t in tolerances:
+        sets += [[(t, float(t.delta))], [(t, -float(t.delta))]]
+    rec, ww, fw = _tol_records(opt_model, sets, num_rays, fields, wvls, foc, table, device, backend, trace_kwargs)
+    return Sensitivity(tolerances, tol_merit(rec, ww, fw, compensate_focus))
+
+
+def tolerance_monte_carlo(opt_model, tolerances, num_trials=1000, seed=0, distribution='normal', num_rays=32,
+                          fields=None, wvls=None, foc=None, compensate_focus=True, table=None, device=0,
+                          backend=None, **trace_kwargs):
+    """Spot merit of ``num_trials`` randomly built systems: every trial draws every tolerance
+    (``draw_tolerances``), and all trials (with the nominal system as variant 0) are traced over the
+    nominal grid in one launch per batch.  Merit, focus compensation and ``backend`` as
+    ``tolerance_sensitivity``.  The same seed gives the same result."""
+    from . import tolerance as TOL
+    for t in tolerances:
+        TOL.check(opt_model.seq_model, t)
+    values = draw_tolerances(tolerances, num_trials, seed, distribution)
+    sets = [[]] + [list(zip(tolerances, row)) for row in values]
+    rec, ww, fw = _tol_records(opt_model, sets, num_rays, fields, wvls, foc, table, device, backend, trace_kwargs)
+    return MonteCarlo(tolerances, values, tol_merit(rec, ww, fw, compensate_focus))

@@ -20,6 +20,8 @@
  *                               shifts (rt_mtf.cuh)
  *   k_trace_grid[_lean]_opd_focus  one trace, the OPD of every ray against up to RT_MAX_FOCUS
  *                               reference spheres (rt_refocus.cuh)
+ *   k_trace_grid_variants       the whole grid traced once per perturbed prescription of a
+ *                               variant set, per-item records (rt_tol.cuh); k_reduce_tol
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
  * The surface table (n_ifc x rt_surface_desc + n_wvl x n_ifc indices) is staged
@@ -44,6 +46,7 @@
 #include "rt_aim.cuh"
 #include "rt_mtf.cuh"
 #include "rt_refocus.cuh"
+#include "rt_tol.cuh"
 
 using namespace b200rt;
 
@@ -129,6 +132,17 @@ struct rt_grid {
     cudaStream_t side[2];
     cudaEvent_t ev_in, ev_side[2];
     bool side_ok;
+};
+
+/* the prescriptions of a tolerance analysis: n_var surface tables of one shape in one allocation */
+struct rt_variants {
+    int32_t device, n_ifc, n_wvl, n_var, sm_count;
+    rt_surface_desc *d_surfs;           /* [n_var][n_ifc] */
+    double *d_n;                        /* [n_var][n_wvl][n_ifc] */
+    double *d_wvl;                      /* [n_wvl] wavelengths in nm (NaN when not given) */
+    unsigned long long *d_counters;     /* ring of RT_COUNTERS work counters */
+    void *d_block;
+    std::atomic<unsigned> next_counter;
 };
 
 /* what the grid kernel needs, passed by value */
@@ -515,20 +529,29 @@ struct RefocusPlanes {
     int32_t n, pad_;
 };
 
+/* the perturbed prescriptions of one rt_trace_grid_variants launch */
+struct VariantPlan {
+    double *items;              /* DEVICE [n_var][n_tiles][chunks_per_tile*RT_WARPS][RT_TOL_DOUBLES] */
+    int32_t n_var, pad_;
+};
+
 /* chunk loop shared by the general and the lean grid kernels: start ray ->
  * trace -> per-ray results -> transverse aberration (focus_pupil_coords,
  * analyses.py:561-580) -> spot sums.  FOCUS: the spot sums of the planes of *FP instead
  * (needs SUMMARY == false and a work counter).  WFE: the wavefront-error sums of wfe_item instead
  * (needs WAVE, SUMMARY == false and a work counter).  OPDF: the OPD against every sphere of *RP
- * instead of out.opd (needs WAVE alone).  NRML: see store_result. */
+ * instead of out.opd (needs WAVE alone).  NRML: see store_result.  VARIANTS: the chunk range once per prescription of *VP,
+ * work item u of variant u / (items of the range); trace gets the variant as a seventh argument; no
+ * per-ray outputs; the item's tol_item record instead (needs a work counter and nothing else). */
 template <bool SUMMARY, bool WAVE, bool FOCUS = false, bool NRML = true, bool WFE = false, bool OPDF = false,
-          typename TraceFn>
+          bool VARIANTS = false, typename TraceFn>
 __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_begin, int64_t chunk_end,
                                                 const rt_out &out, double *scratch, double *acc,
                                                 unsigned long long *work_counter, double *item_sums,
                                                 TraceFn trace, const FocusPlanes *FP = nullptr,
-                                                const RefocusPlanes *RP = nullptr)
+                                                const RefocusPlanes *RP = nullptr, const VariantPlan *VP = nullptr)
 {
+    static_assert(!VARIANTS || (!SUMMARY && !WAVE && !FOCUS && !WFE && !OPDF), "VARIANTS writes its own records");
     static_assert(!WFE || (WAVE && !SUMMARY && !FOCUS), "WFE needs the OPD epilogue and no spot sums");
     static_assert(!OPDF || (WAVE && !SUMMARY && !FOCUS && !WFE), "OPDF needs the OPD epilogue alone");
     const int64_t tile0 = chunk_begin/G.chunks_per_tile;
@@ -537,8 +560,10 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
     const bool chunk_slots = FOCUS ? FP->chunk_slots != 0 : G.chunks_per_tile <= (int64_t)gridDim.x;
     int64_t cur_tile = -1;
     if (SUMMARY && !chunk_slots) acc_init(acc);
-    const unsigned long long n_items = (unsigned long long)(chunk_end - chunk_begin)*RT_WARPS;
+    const unsigned long long per_var = (unsigned long long)(chunk_end - chunk_begin)*RT_WARPS;
+    const unsigned long long n_items = VARIANTS ? per_var*(unsigned long long)VP->n_var : per_var;
     int64_t c = chunk_begin + blockIdx.x;
+    int var = 0;
     for (;;) {
         int slice;                       /* which 32 rays of the chunk this warp takes */
         unsigned long long item = 0;
@@ -550,8 +575,13 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             if ((threadIdx.x & 31) == 0) u = atomicAdd(work_counter, 1ull);
             u = __shfl_sync(0xffffffffu, u, 0);
             if (u >= n_items) break;
-            c = chunk_begin + (int64_t)(u/RT_WARPS);
-            slice = (int)(u % RT_WARPS);
+            unsigned long long r = u;
+            if (VARIANTS) {
+                var = (int)(u/per_var);
+                r = u - (unsigned long long)var*per_var;
+            }
+            c = chunk_begin + (int64_t)(r/RT_WARPS);
+            slice = (int)(r % RT_WARPS);
             item = u;
         } else {
             if (c >= chunk_end) break;
@@ -577,10 +607,11 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             const int64_t k = tile*G.rays_per_tile + loc - ray0;
             RayResult R;
             Vec3 d0;
-            trace(f, w, loc, k, R, d0);
-            store_result<NRML>(out, k, R);
+            if constexpr (VARIANTS) trace(f, w, loc, k, R, d0, var);
+            else trace(f, w, loc, k, R, d0);
+            if (!VARIANTS) store_result<NRML>(out, k, R);
             status = R.status; op = R.op;
-            if (FOCUS) { fp = R.p; fd = R.d; }
+            if (FOCUS || VARIANTS) { fp = R.p; fd = R.d; }
             if (OPDF) {
                 /* every plane of the ray: the sphere records of a work item's tile are warp-uniform loads */
                 double *dst = RP->planes + k;
@@ -602,13 +633,13 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
                     grid_pupil_coords(G, f, loc, wx, wy);
                 }
             }
-            if (out.abr_x || SUMMARY) {
+            if (VARIANTS || out.abr_x || SUMMARY) {
                 const double rx = G.ref_img ? G.ref_img[tile*2 + 0] : 0.0;
                 const double ry = G.ref_img ? G.ref_img[tile*2 + 1] : 0.0;
                 double dist = div_maybe_zero(G.foc, R.d.z);
                 ax = (R.p.x + dist*R.d.x) - rx;
                 ay = (R.p.y + dist*R.d.y) - ry;
-                if (out.abr_x) {
+                if (!VARIANTS && out.abr_x) {
                     double sx = ax, sy = ay;
                     if ((out.flags & RT_OUT_ABR_NAN_STATUS) && status != RT_RAY_OK) {
                         sx = __longlong_as_double((long long)(RT_NAN_PAYLOAD_BASE | (unsigned long long)(status & 0xFFFF)));
@@ -639,6 +670,8 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             cur_tile = tile;
             wfe_item(have, status, wW, wx, wy, tile, first, sl, scratch, item_sums + item*RT_WFE_ITEM_SUMS);
         }
+        /* a variant's items are its tiles' items in order: item u is record u */
+        if (VARIANTS) tol_item(have, status, ax, ay, op, fd, VP->items + item*RT_TOL_DOUBLES);
         if (!work_counter) c += gridDim.x;
     }
     if (SUMMARY && !chunk_slots && cur_tile >= 0) acc_flush(acc, scratch, cur_tile, blockIdx.x, sl);
@@ -737,6 +770,28 @@ k_trace_grid_opd_focus(const rt_surface_desc *__restrict__ g_surfs, const double
             const int wi = G.wvl_idx[w];
             trace_ray<false, true>(tab, ntab + (int64_t)wi*n_ifc, g_wvl[wi], n_ifc, o, p0, d0, fw, R);
         }, nullptr, &P);
+}
+
+/* every prescription of a variant set over the whole grid (rt_trace_grid_variants): the general
+ * trace with the table read from global memory, since a warp's prescription changes from one work
+ * item to the next.  g_surfs / g_n: the set's rows from the launch's first variant on */
+__global__ void __launch_bounds__(RT_BLOCK)
+k_trace_grid_variants(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                      int n_ifc, int n_wvl, GridDev G, int64_t n_chunks, rt_opts o,
+                      const double *__restrict__ g_wvl, int pupil_kind, unsigned long long *work_counter,
+                      VariantPlan P)
+{
+    const rt_out out = {};
+    grid_chunk_loop<false, false, false, false, false, false, true>(G, 0, n_chunks, out, nullptr, nullptr,
+                                                                    work_counter, nullptr,
+        [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0, int v) {
+            Vec3 p0;
+            grid_start_ray<false>(G, pupil_kind, f, loc, p0, d0);
+            FullWriter fw = {nullptr, 0};
+            const int wi = G.wvl_idx[w];
+            trace_ray<false, false>(g_surfs + (int64_t)v*n_ifc, g_n + ((int64_t)v*n_wvl + wi)*n_ifc, g_wvl[wi],
+                                    n_ifc, o, p0, d0, fw, R);
+        }, nullptr, nullptr, &P);
 }
 
 /* ---- lean kernels: plan built in shared memory by the CTA (rt_lean.cuh) */
@@ -949,6 +1004,13 @@ struct WfeLayout {         /* RT_WFE_DOUBLES: wavefront-error sums */
     static __device__ __forceinline__ constexpr int item_col(int j) { return 7 + j; }
 };
 
+struct TolLayout {         /* RT_TOL_DOUBLES: tolerance records; the records are work items */
+    static constexpr int W = RT_TOL_DOUBLES, ACC = RT_TOL_VALID, N_ITEM = 1, SH = RT_TOL_VALID + 1;  /* no item sums */
+    static __device__ __forceinline__ constexpr bool is_min(int k) { return k == 10 || k == 12; }
+    static __device__ __forceinline__ constexpr bool is_max(int k) { return k == 11 || k == 13; }
+    static __device__ __forceinline__ constexpr int item_col(int j) { return j; }
+};
+
 template <typename L>
 __device__ __forceinline__ double red_op(int k, double a, double y)
 {
@@ -1074,6 +1136,15 @@ k_reduce_wfe(const double *__restrict__ scratch, int64_t recs_per_tile, double *
 {
     reduce_tile<WfeLayout, false>(scratch, recs_per_tile, partials, tickets, summary, item_sums, chunk_begin,
                                   chunk_end, chunks_per_tile, 0, 0);
+}
+
+/* k_reduce_summary for the per-item records of rt_trace_grid_variants: one summary tile per (variant,
+ * grid tile), whose records are its work items in item order */
+__global__ void __launch_bounds__(RT_RED_THREADS)
+k_reduce_tol(const double *__restrict__ items, int64_t items_per_tile, double *partials, unsigned int *tickets,
+             double *__restrict__ record)
+{
+    reduce_tile<TolLayout, false>(items, items_per_tile, partials, tickets, record, nullptr, 0, 0, 1, 0, 0);
 }
 
 /* summary of an empty chunk range: zero counts / sums, identities in the min / max columns */
@@ -1676,6 +1747,26 @@ static GridDev grid_dev(const rt_grid *g)
     return G;
 }
 
+/* the descriptor fields the kernels index or switch on, for rt_table_create / rt_variants_create */
+static int check_descs(const char *fn, const rt_surface_desc *surfs, int64_t n)
+{
+    for (int64_t i = 0; i < n; i++) {
+        const rt_surface_desc &s = surfs[i];
+        if (s.profile < RT_PROFILE_SPHERICAL || s.profile > RT_PROFILE_THINLENS)
+            return fail(RT_ERR_UNSUPPORTED, "%s: unknown profile id", fn);
+        if (s.mode < RT_MODE_TRANSMIT || s.mode > RT_MODE_PHANTOM)
+            return fail(RT_ERR_UNSUPPORTED, "%s: unknown interact mode", fn);
+        if (s.n_coefs < 0 || s.n_coefs > RT_MAX_COEFS || s.n_apertures < 0 ||
+            s.n_apertures > RT_MAX_APERTURES)
+            return fail(RT_ERR_INVALID, "%s: coefficient / aperture count out of range", fn);
+        if (s.phase_kind < RT_PHASE_NONE || s.phase_kind > RT_PHASE_RADIAL)
+            return fail(RT_ERR_UNSUPPORTED, "%s: unknown phase element kind", fn);
+        if (s.n_phase_coefs < 0 || s.n_phase_coefs > RT_MAX_PHASE_COEFS)
+            return fail(RT_ERR_INVALID, "%s: phase coefficient count out of range", fn);
+    }
+    return RT_OK;
+}
+
 /* ------------------------------------------------------------------ C ABI */
 extern "C" {
 
@@ -1689,20 +1780,8 @@ int rt_table_create(const rt_surface_desc *surfs, int32_t n_ifc, const double *n
 {
     if (!surfs || !n_by_wvl || !out || n_ifc < 2 || n_wvl < 1)
         return fail(RT_ERR_INVALID, "rt_table_create: bad arguments");
-    for (int i = 0; i < n_ifc; i++) {
-        const rt_surface_desc &s = surfs[i];
-        if (s.profile < RT_PROFILE_SPHERICAL || s.profile > RT_PROFILE_THINLENS)
-            return fail(RT_ERR_UNSUPPORTED, "rt_table_create: unknown profile id");
-        if (s.mode < RT_MODE_TRANSMIT || s.mode > RT_MODE_PHANTOM)
-            return fail(RT_ERR_UNSUPPORTED, "rt_table_create: unknown interact mode");
-        if (s.n_coefs < 0 || s.n_coefs > RT_MAX_COEFS || s.n_apertures < 0 ||
-            s.n_apertures > RT_MAX_APERTURES)
-            return fail(RT_ERR_INVALID, "rt_table_create: coefficient / aperture count out of range");
-        if (s.phase_kind < RT_PHASE_NONE || s.phase_kind > RT_PHASE_RADIAL)
-            return fail(RT_ERR_UNSUPPORTED, "rt_table_create: unknown phase element kind");
-        if (s.n_phase_coefs < 0 || s.n_phase_coefs > RT_MAX_PHASE_COEFS)
-            return fail(RT_ERR_INVALID, "rt_table_create: phase coefficient count out of range");
-    }
+    int rc = check_descs("rt_table_create", surfs, n_ifc);
+    if (rc) return rc;
     DeviceGuard guard(device);
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
@@ -2390,6 +2469,114 @@ int rt_trace_grid_wfe(const rt_table *t, const rt_grid *g, int64_t chunk_begin, 
     if (rc) return rc;
     k_reduce_wfe<<<(unsigned)(g->n_tiles*RT_RED_SPLIT), RT_RED_THREADS, 0, s>>>(
         scr, recs/g->n_tiles, partials, tickets, summary, items, chunk_begin, chunk_end, g->chunks_per_tile);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
+}
+
+/* ---- tolerance analysis: many prescriptions over one grid */
+int rt_variants_create(const rt_surface_desc *surfs, int32_t n_ifc, const double *n_by_wvl, int32_t n_wvl,
+                       int32_t n_var, const double *wvl_nm, int32_t device, rt_variants **out)
+{
+    if (!surfs || !n_by_wvl || !out || n_ifc < 2 || n_wvl < 1 || n_var < 1)
+        return fail(RT_ERR_INVALID, "rt_variants_create: bad arguments");
+    int rc = check_descs("rt_variants_create", surfs, (int64_t)n_var*n_ifc);
+    if (rc) return rc;
+    DeviceGuard guard(device);
+    cudaDeviceProp prop;
+    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
+    const size_t b_s = (size_t)n_var*n_ifc*sizeof(rt_surface_desc);
+    const size_t b_n = (size_t)n_var*n_wvl*n_ifc*sizeof(double), b_w = (size_t)n_wvl*sizeof(double);
+    const size_t b_c = RT_COUNTERS*sizeof(unsigned long long);
+    std::vector<unsigned char> h(b_s + b_n + b_w);
+    memcpy(h.data(), surfs, b_s);
+    memcpy(h.data() + b_s, n_by_wvl, b_n);
+    for (int32_t w = 0; w < n_wvl; w++) {
+        const double x = wvl_nm ? wvl_nm[w] : (double)NAN;
+        memcpy(h.data() + b_s + b_n + (size_t)w*sizeof(double), &x, sizeof(double));
+    }
+    rt_variants *v = new (std::nothrow) rt_variants();
+    if (!v) return fail(RT_ERR_NOMEM, "rt_variants_create: out of host memory");
+    v->device = device; v->n_ifc = n_ifc; v->n_wvl = n_wvl; v->n_var = n_var;
+    v->sm_count = prop.multiProcessorCount;
+    v->d_block = nullptr; v->next_counter = 0;
+    cudaError_t e = cudaMalloc(&v->d_block, h.size() + b_c);
+    if (e == cudaSuccess) e = cudaMemcpy(v->d_block, h.data(), h.size(), cudaMemcpyHostToDevice);
+    /* pageable copies: see rt_grid_create */
+    if (e == cudaSuccess) e = cudaStreamSynchronize(cudaStreamLegacy);
+    if (e != cudaSuccess) {
+        cudaFree(v->d_block); delete v;
+        return fail(RT_ERR_CUDA, "rt_variants_create: %s", cudaGetErrorString(e));
+    }
+    unsigned char *base = (unsigned char *)v->d_block;
+    v->d_surfs = (rt_surface_desc *)base;
+    v->d_n = (double *)(base + b_s);
+    v->d_wvl = (double *)(base + b_s + b_n);
+    v->d_counters = (unsigned long long *)(base + b_s + b_n + b_w);
+    *out = v;
+    return RT_OK;
+}
+
+int rt_variants_destroy(rt_variants *v)
+{
+    if (!v) return RT_OK;
+    DeviceGuard guard(v->device);
+    cudaFree(v->d_block);
+    delete v;
+    return RT_OK;
+}
+
+/* scratch of rt_trace_grid_variants over n_var variants: item records [n_var][n_tiles][chunks_per_tile*RT_WARPS]
+ * [RT_TOL_DOUBLES] | partials [n_var*n_tiles][RT_RED_SPLIT][RT_TOL_DOUBLES] | tickets [n_var*n_tiles] */
+static int64_t tol_items(const rt_grid *g, int64_t n_var) { return n_var*g->n_chunks*RT_WARPS; }
+
+int64_t rt_grid_variants_scratch_bytes(const rt_grid *g, int32_t n_var)
+{
+    if (!g || n_var < 0) return 0;
+    const int64_t tiles = (int64_t)n_var*g->n_tiles;
+    return ((tol_items(g, n_var) + tiles*RT_RED_SPLIT)*RT_TOL_DOUBLES + (tiles + 1)/2)*(int64_t)sizeof(double);
+}
+
+int rt_trace_grid_variants(const rt_variants *v, const rt_grid *g, int32_t var_begin, int32_t var_end,
+                           const rt_opts *o, double *record, void *scratch, void *stream)
+{
+    if (!v || !g || !o) return fail(RT_ERR_INVALID, "rt_trace_grid_variants: bad arguments");
+    if (var_begin < 0 || var_end > v->n_var || var_end < var_begin)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_variants: variant range out of bounds");
+    if (var_end > var_begin && (!record || !scratch))
+        return fail(RT_ERR_INVALID, "rt_trace_grid_variants: record and scratch are required");
+    if (v->device != g->device)
+        return fail(RT_ERR_INVALID, "rt_trace_grid_variants: variants and grid on different devices");
+    if (o->wvl_idx < 0 || o->wvl_idx >= v->n_wvl) return fail(RT_ERR_INVALID, "opts.wvl_idx out of range");
+    for (int32_t wi : g->h_wvl_idx)
+        if (wi < 0 || wi >= v->n_wvl)
+            return fail(RT_ERR_INVALID, "rt_trace_grid_variants: the grid's wvl_idx is out of range for the variants");
+    if (var_end == var_begin) return RT_OK;
+    DeviceGuard guard(v->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const int32_t n_var = var_end - var_begin;
+    const int64_t tiles = (int64_t)n_var*g->n_tiles;
+    double *items = (double *)scratch;
+    double *partials = items + tol_items(g, n_var)*RT_TOL_DOUBLES;
+    unsigned int *tickets = (unsigned int *)(partials + tiles*RT_RED_SPLIT*RT_TOL_DOUBLES);
+    /* every item record is written by the trace and every partial before it is read: clear the tickets */
+    CUDA_TRY(cudaMemsetAsync(tickets, 0, (size_t)tiles*sizeof(unsigned int), s));
+    rt_variants *vv = const_cast<rt_variants *>(v);
+    unsigned long long *wc = v->d_counters + (vv->next_counter++ % RT_COUNTERS);
+    CUDA_TRY(cudaMemsetAsync(wc, 0, sizeof(unsigned long long), s));
+    VariantPlan P;
+    P.items = items; P.n_var = n_var; P.pad_ = 0;
+    int grid;
+    int rc = persistent_grid(k_trace_grid_variants, 0, v->sm_count, tol_items(g, n_var)/RT_WARPS, &grid);
+    if (rc) return rc;
+    k_trace_grid_variants<<<grid, RT_BLOCK, 0, s>>>(v->d_surfs + (int64_t)var_begin*v->n_ifc,
+                                                    v->d_n + (int64_t)var_begin*v->n_wvl*v->n_ifc, v->n_ifc,
+                                                    v->n_wvl, grid_dev(g), g->n_chunks, *o, v->d_wvl,
+                                                    g->pupil_kind, wc, P);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    k_reduce_tol<<<(unsigned)(tiles*RT_RED_SPLIT), RT_RED_THREADS, 0, s>>>(
+        items, g->chunks_per_tile*RT_WARPS, partials, tickets, record);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RT_OK;

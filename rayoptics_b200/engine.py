@@ -20,7 +20,8 @@ import torch
 
 from . import _abi
 from ._abi import (rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES, RT_WFE_DOUBLES,
-                   RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS, RT_MTF_DOUBLES, RT_MTF_MAX_RAYS, RT_SPHERE_DOUBLES)
+                   RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS, RT_MTF_DOUBLES, RT_MTF_MAX_RAYS, RT_SPHERE_DOUBLES,
+                   RT_TOL_DOUBLES)
 
 SUMMARY_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other',
                   'sum_x', 'sum_y', 'sum_xx', 'sum_yy', 'sum_xy',
@@ -994,6 +995,98 @@ def measure_fp64_latency(device=0):
     v = C.c_double()
     _abi.check(lib.rt_measure_fp64_latency(int(device), C.byref(v)))
     return v.value
+
+
+# columns of a tolerance record (RT_TOL_DOUBLES, include/b200rt.h): the spot summary, then the sums of
+# the last segment's slopes ux = dx/dz, uy = dy/dz that move the spot with the focus
+TOL_FIELDS = SUMMARY_FIELDS + ('sum_ux', 'sum_uy', 'sum_uxux', 'sum_uyuy', 'sum_xux', 'sum_yuy',
+                               'reserved0', 'reserved1')
+# scratch of one trace_grid_variants launch is ~6 B per ray and variant; larger sets go in batches
+VARIANT_SCRATCH_CAP = 1 << 30
+
+
+class VariantSet:
+    """``n_var`` surface tables of one shape on the device (``rt_variants*``): ``descs`` is a
+    sequence of ``rt_surface_desc`` arrays (or one array of ``n_var * n_ifc``), ``n_by_wvl``
+    ``[n_var, n_wvl, n_ifc]``.  One allocation and one copy; immutable."""
+
+    def __init__(self, descs, n_by_wvl, wvls=None, device=0):
+        lib = _abi.load_library()
+        self.n_by_wvl = np.ascontiguousarray(n_by_wvl, dtype=np.float64)
+        self.n_var, self.n_wvl, self.n_ifc = self.n_by_wvl.shape
+        if isinstance(descs, C.Array) and len(descs) == self.n_var*self.n_ifc:
+            flat = descs
+        else:
+            flat = (_abi.rt_surface_desc*(self.n_var*self.n_ifc))()
+            size = C.sizeof(_abi.rt_surface_desc)*self.n_ifc
+            for v, d in enumerate(descs):
+                if len(d) != self.n_ifc:
+                    raise ValueError('every variant needs n_ifc descriptors')
+                C.memmove(C.addressof(flat) + v*size, d, size)
+        w = None
+        if wvls is not None and all(isinstance(x, (int, float)) for x in wvls):
+            w = np.ascontiguousarray(wvls, dtype=np.float64)
+        self.device = int(device)
+        handle = C.c_void_p()
+        _abi.check(lib.rt_variants_create(flat, self.n_ifc, self.n_by_wvl.ctypes.data_as(_abi.c_double_p),
+                                          self.n_wvl, self.n_var,
+                                          None if w is None else w.ctypes.data_as(_abi.c_double_p),
+                                          self.device, C.byref(handle)))
+        self._handle, self._lib = handle, lib
+
+    @property
+    def handle(self):
+        if self._handle is None:
+            raise RuntimeError('VariantSet was destroyed')
+        return self._handle
+
+    def close(self):
+        if getattr(self, '_handle', None) is not None:
+            self._lib.rt_variants_destroy(self._handle)
+            self._handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def variant_batch(grid, n_var, cap=VARIANT_SCRATCH_CAP):
+    """variants per ``rt_trace_grid_variants`` launch so that its scratch stays under ``cap`` bytes"""
+    lib = _abi.load_library()
+    per = max(1, int(lib.rt_grid_variants_scratch_bytes(grid.handle, 1)))
+    return max(1, min(int(n_var), cap//per))
+
+
+def trace_grid_variants(variants, grid, var_begin=0, var_end=None, cap=VARIANT_SCRATCH_CAP, **kwargs):
+    """Tolerance records of variants ``[var_begin, var_end)`` of a VariantSet over the whole
+    PupilGrid (``rt_trace_grid_variants``): ``[n, n_tiles, RT_TOL_DOUBLES]`` float64 device tensor
+    (TOL_FIELDS).  The variants go in batches whose scratch stays under ``cap`` bytes (two launches
+    per batch).  Trace defaults as ``trace_grid``.  Asynchronous on the current CUDA stream."""
+    lib = _abi.load_library()
+    device = torch.device('cuda', variants.device)
+    var_end = variants.n_var if var_end is None else int(var_end)
+    kwargs.setdefault('check_apertures', True)
+    kwargs.setdefault('first_surf', 1)
+    kwargs.setdefault('last_surf', variants.n_ifc - 2)
+    if grid.pupil_kind == _abi.PUPIL_WIDE:
+        kwargs['intersect_obj'] = False
+    opts = _abi.make_opts(**kwargs)
+    n = max(var_end - int(var_begin), 0)
+    rec = torch.empty((n, grid.n_tiles, RT_TOL_DOUBLES), dtype=torch.float64, device=device)
+    if n == 0:
+        return rec
+    batch = variant_batch(grid, n, cap)
+    scratch = torch.empty(max(int(lib.rt_grid_variants_scratch_bytes(grid.handle, batch))//8, 1),
+                          dtype=torch.float64, device=device)
+    stream = _stream_ptr(device)
+    for v0 in range(int(var_begin), var_end, batch):
+        v1 = min(v0 + batch, var_end)
+        _abi.check(lib.rt_trace_grid_variants(variants.handle, grid.handle, v0, v1, C.byref(opts),
+                                              _ptr(rec[v0 - var_begin]), _ptr(scratch), stream))
+    rec._keep = scratch            # scratch must outlive the asynchronous launches
+    return rec
 
 
 def launch_count():

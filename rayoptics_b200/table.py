@@ -23,6 +23,31 @@ class _ThinLensProfile:
     cv = 0.0
 
 
+def profile_fields(profile, pname):
+    """``(cv, cc, ec)`` of a profile as the table stores them"""
+    if pname in ('Spherical', 'ThinLens'):
+        return float(profile.cv), 0.0, 1.0
+    return float(profile.cv), float(profile.cc), float(profile.ec)
+
+
+def set_transform(d, tfrm):
+    """``rt``, ``t`` and ``has_tfrm`` of descriptor ``d`` from a path transform ``(rt, t)`` or None"""
+    if tfrm is None:
+        rt, t = np.identity(3), np.zeros(3)
+    else:
+        rt, t = np.asarray(tfrm[0], dtype=float), np.asarray(tfrm[1], dtype=float)
+    if np.array_equal(rt, np.identity(3)):
+        d.has_tfrm = 0
+    elif rt.flags['C_CONTIGUOUS'] and not rt.flags['F_CONTIGUOUS']:
+        d.has_tfrm = 2   # numpy takes the dgemv 't' path for rt.dot(v)
+    else:
+        d.has_tfrm = 1   # r.transpose() of a C array (elem/transform.py:86)
+    for i in range(9):
+        d.rt[i] = float(rt.reshape(-1)[i])
+    for i in range(3):
+        d.t[i] = float(t[i])
+
+
 class UnsupportedInterfaceError(NotImplementedError):
     """The model contains an interface the table cannot represent (thin lens,
     diffractive/holographic phase element, user subclass ...)."""
@@ -79,11 +104,7 @@ def _describe_interface(seg, prev_n, prev_zdir):
     # raytrace.py:212-221: any unknown interact_mode passes the ray through
     d.mode = MODE_IDS.get(getattr(ifc, 'interact_mode', 'dummy'), MODE_IDS['dummy'])
     d.z_dir = int(z_dir if z_dir is not None else prev_zdir)
-    d.cv = float(profile.cv)
-    if pname in ('Spherical', 'ThinLens'):
-        d.cc, d.ec = 0.0, 1.0
-    else:
-        d.cc, d.ec = float(profile.cc), float(profile.ec)
+    d.cv, d.cc, d.ec = profile_fields(profile, pname)
     d.cR = float(getattr(profile, 'cR', 0.0))
     coefs = list(getattr(profile, 'coefs', []))
     k = getattr(profile, 'max_nonzero_coef', None)
@@ -114,20 +135,7 @@ def _describe_interface(seg, prev_n, prev_zdir):
         else:
             a.a, a.b = float(ca.x_half_width), float(ca.y_half_width)
         a.x_offset, a.y_offset = float(ca.x_offset), float(ca.y_offset)
-    if tfrm is None:
-        rt, t = np.identity(3), np.zeros(3)
-    else:
-        rt, t = np.asarray(tfrm[0], dtype=float), np.asarray(tfrm[1], dtype=float)
-    if np.array_equal(rt, np.identity(3)):
-        d.has_tfrm = 0
-    elif rt.flags['C_CONTIGUOUS'] and not rt.flags['F_CONTIGUOUS']:
-        d.has_tfrm = 2   # numpy takes the dgemv 't' path for rt.dot(v)
-    else:
-        d.has_tfrm = 1   # r.transpose() of a C array (elem/transform.py:86)
-    for i in range(9):
-        d.rt[i] = float(rt.reshape(-1)[i])
-    for i in range(3):
-        d.t[i] = float(t[i])
+    set_transform(d, tfrm)
     return d, float(n if n is not None else prev_n), d.z_dir
 
 
