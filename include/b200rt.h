@@ -531,6 +531,38 @@ int64_t rt_grid_variants_scratch_bytes(const rt_grid *grid, int32_t n_var);
  * range.  Two launches on `stream` (none for an empty range). */
 int rt_trace_grid_variants(const rt_variants *variants, const rt_grid *grid, int32_t var_begin, int32_t var_end,
                            const rt_opts *opts, double *record, void *scratch, void *stream);
+/* The wave records of every variant of [var_begin, var_end) and grid tile, built on the device (one
+ * thread per (variant, tile)): the chief ray of rt_grid_chief_ref (pupil (0, 0) of the grid's pupil
+ * kind, no vignetting, apertures not checked, first_surf 1, last_surf n_ifc - 2) traced at the tile's
+ * wavelength through the variant's rows, then the exit pupil, reference sphere at the grid's foc and
+ * record of rayoptics_b200/waveabr.py (transfer_to_exit_pupil, calculate_reference_sphere with its own
+ * chief-ray image point, wave_record; csrc/rt_tolwave.cuh).  The image gap's thickness and the last
+ * local transform are the variant's own descriptor n_ifc - 2; the paraxial data is nominal:
+ *   parax: HOST [3] = fod.exp_dist, |fod.n_obj|, |fod.n_img|
+ *   wave: DEVICE [var_end - var_begin][n_tiles][RT_WAVE_DOUBLES] (the rt_grid_spec.wave layout)
+ *   ref_img: DEVICE [..][n_tiles][2] the chief rays' image points at foc
+ *   status: DEVICE [..][n_tiles] the chief rays' rt_status; a chief ray that does not reach the image
+ *           gives its (variant, tile) an all-NaN record and reference point (not an error)
+ * RT_ERR_INVALID as rt_trace_grid_variants; RT_ERR_UNSUPPORTED where rt_trace_grid_wfe refuses the OPD
+ * (< 3 interfaces, or a decenter on interface n_ifc - 2) in any variant of the range.  Both before
+ * any device work.  One launch on `stream` (none for an empty range). */
+int rt_variants_wave(const rt_variants *variants, const rt_grid *grid, int32_t var_begin, int32_t var_end,
+                     const double *parax, double *wave, double *ref_img, int32_t *status, void *stream);
+/* bytes of scratch rt_trace_grid_variants_wfe needs for n_var variants */
+int64_t rt_grid_variants_wfe_scratch_bytes(const rt_grid *grid, int32_t n_var);
+/* rt_trace_grid_variants with the wavefront-error epilogue: each ray's OPD against its variant's wave
+ * record (wave: DEVICE [var_end - var_begin][n_tiles][RT_WAVE_DOUBLES], e.g. rt_variants_wave's), the
+ * grid's own wave records and reference points unused.
+ * record: DEVICE [var_end - var_begin][n_tiles][RT_WFE_DOUBLES], rt_trace_grid_wfe's summary layout
+ * (0-4 counts, 5 / 6 min / max W, 7-19 the 13 sums, 20-23 zero); equal, bit for bit, to
+ * rt_trace_grid_wfe's summary for a table of that variant alone on a grid carrying that variant's wave
+ * records (dynamic schedule).  Sum order (DESIGN.md section 4): the 13 summands of every work item added
+ * by the halving tree of rt_trace_grid_wfe, reduce_tile over a (variant, tile)'s items in item order.
+ * Errors as rt_trace_grid_variants, plus RT_ERR_INVALID for a NULL wave and RT_ERR_UNSUPPORTED as
+ * rt_variants_wave, before any device work.  Two launches on `stream` (none for an empty range). */
+int rt_trace_grid_variants_wfe(const rt_variants *variants, const rt_grid *grid, int32_t var_begin,
+                               int32_t var_end, const rt_opts *opts, const double *wave, double *record,
+                               void *scratch, void *stream);
 
 /* ---- misc */
 const char *rt_last_error(void);

@@ -130,7 +130,8 @@ EXPORTS = ['rt_table_create', 'rt_table_destroy', 'rt_table_dims', 'rt_table_set
            'rt_trace_grid_focus', 'rt_grid_wfe_scratch_bytes', 'rt_trace_grid_wfe', 'rt_combine_wfe',
            'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike', 'rt_grid_aim_chief',
            'rt_grid_pupil_function', 'rt_grid_mtf', 'rt_grid_mtf_shifts', 'rt_trace_grid_opd_focus',
-           'rt_variants_create', 'rt_variants_destroy', 'rt_grid_variants_scratch_bytes', 'rt_trace_grid_variants']
+           'rt_variants_create', 'rt_variants_destroy', 'rt_grid_variants_scratch_bytes', 'rt_trace_grid_variants',
+           'rt_variants_wave', 'rt_grid_variants_wfe_scratch_bytes', 'rt_trace_grid_variants_wfe']
 
 _lib = None
 
@@ -223,6 +224,12 @@ def load_library():
     lib.rt_grid_variants_scratch_bytes.restype = i64
     lib.rt_trace_grid_variants.argtypes = [vp, vp, i32, i32, C.POINTER(rt_opts), vp, vp, vp]
     lib.rt_trace_grid_variants.restype = i32
+    lib.rt_variants_wave.argtypes = [vp, vp, i32, i32, c_double_p, vp, vp, vp, vp]
+    lib.rt_variants_wave.restype = i32
+    lib.rt_grid_variants_wfe_scratch_bytes.argtypes = [vp, i32]
+    lib.rt_grid_variants_wfe_scratch_bytes.restype = i64
+    lib.rt_trace_grid_variants_wfe.argtypes = [vp, vp, i32, i32, C.POINTER(rt_opts), vp, vp, vp, vp]
+    lib.rt_trace_grid_variants_wfe.restype = i32
     lib.rt_last_error.restype = C.c_char_p
     lib.rt_abi_version.restype = i32
     lib.rt_chunk_rays.restype = i32

@@ -1598,15 +1598,61 @@ def tol_merit(rec, wvl_wts, field_wts, compensate_focus=True):
     return TolMerit(merit_at(focus), focus, merit_at(np.zeros(len(focus))), rec[..., 0].sum(axis=2), cen)
 
 
+class WaveMerit:
+    """The wavefront merit of every variant of a tolerance run (``wave_merit``), in waves: ``merit``
+    ``[n_var]`` M; ``sigma`` / ``strehl`` ``[n_var, n_fields]`` the polychromatic RMS wavefront error
+    sigma_f and its Marechal Strehl ratio exp(-(2 pi sigma_f)^2); ``n_ok`` ``[n_var, n_fields]`` rays that
+    reach the image (all wavelengths); per tile ``[n_var, n_fields, n_wvls]``: ``rms`` the RMS wavefront
+    error the merit uses (tilt and focus removed with the focus compensator, tilt removed without),
+    ``focus`` the fitted focus coefficient on {1, x, y, r^2} (waves at unit relative pupil) and
+    ``chief_status`` the status of the tile's chief ray (a tile whose chief ray fails is NaN)."""
+
+    def __init__(self, merit, sigma, n_ok, rms, focus, chief_status):
+        self.merit, self.sigma, self.n_ok, self.rms, self.focus = merit, sigma, n_ok, rms, focus
+        self.strehl = np.exp(-(2.0*np.pi*sigma)**2)
+        self.chief_status = chief_status
+
+
+def wave_merit_of(rms, wvl_wts, field_wts):
+    """``(M [n_var], sigma_f [n_var, n_fields])`` from per-tile RMS wavefront errors ``rms`` ``[n_var,
+    n_fields, n_wvls]``: sigma_f^2 = sum_w S_w rms_fw^2 / sum_w S_w (spectral weights S), M = sqrt(sum_f
+    W_f sigma_f^2 / sum_f W_f) (field weights W)"""
+    w = np.asarray(wvl_wts, dtype=np.float64)
+    W = np.asarray(field_wts, dtype=np.float64)
+    s2 = (rms*rms*w).sum(axis=2)/w.sum()
+    return np.sqrt((s2*W).sum(axis=1)/W.sum()), np.sqrt(s2)
+
+
+def wave_merit(rec, lam, wvl_wts, field_wts, compensate_focus=True, chief_status=None):
+    """``WaveMerit`` of wavefront-error records ``[n_var, n_fields, n_wvls, RT_WFE_DOUBLES]``
+    (``engine.wavefront_statistics`` per tile; ``lam`` ``[n_wvls]`` the wavelengths in system units).
+    With ``compensate_focus`` each tile's RMS has tilt and focus removed (``rms_focus``): every (field,
+    wavelength) is refocused on its own, which is more optimistic than the spot criterion's one common
+    defocus.  Without it tilt only (``rms_tilt``)."""
+    rec = np.asarray(rec, dtype=np.float64)
+    nv, nf, nw = rec.shape[:3]
+    lam_t = np.broadcast_to(np.asarray(lam, dtype=np.float64)[None, None, :], (nv, nf, nw)).ravel()
+    st = E.wavefront_statistics(rec.reshape(-1, rec.shape[-1]), lam_t)
+    rms = st['rms_focus' if compensate_focus else 'rms_tilt'].reshape(nv, nf, nw)
+    merit, sigma = wave_merit_of(rms, wvl_wts, field_wts)
+    cs = np.zeros((nv, nf, nw), dtype=np.int32) if chief_status is None else np.asarray(chief_status)
+    return WaveMerit(merit, sigma, rec[..., 0].sum(axis=2), rms, st['focus'].reshape(nv, nf, nw), cs)
+
+
 class Sensitivity:
     """Result of ``tolerance_sensitivity``.  ``nominal`` / ``nominal_focus``: M and delta* of the
     nominal system; per tolerance ``merit_plus`` / ``merit_minus`` (at +-delta), ``delta_plus`` /
     ``delta_minus`` (their change of M), ``focus_plus`` / ``focus_minus``; ``estimated`` = M0 +
     sqrt(sum_i max(dM_i+, dM_i-, 0)^2); ``result``: the ``TolMerit`` of every variant (0 nominal,
-    then +delta, -delta per tolerance)."""
+    then +delta, -delta per tolerance).  With the wavefront criterion ``result`` is a ``WaveMerit``,
+    the focus values are its per-tile ``focus`` coefficients and, since wavefront variances add,
+    ``estimated`` = sqrt(M0^2 + sum_i max(M_i+^2 - M0^2, M_i-^2 - M0^2, 0))."""
 
     def __init__(self, tolerances, res):
         self.tolerances, self.result = list(tolerances), res
+        if isinstance(res, WaveMerit):
+            self._init_wave(res)
+            return
         self.nominal, self.nominal_focus = float(res.merit[0]), float(res.focus[0])
         self.merit_plus, self.merit_minus = res.merit[1::2].copy(), res.merit[2::2].copy()
         self.focus_plus, self.focus_minus = res.focus[1::2].copy(), res.focus[2::2].copy()
@@ -1614,11 +1660,23 @@ class Sensitivity:
         worst = np.maximum(np.maximum(self.delta_plus, self.delta_minus), 0.0)
         self.estimated = self.nominal + float(np.sqrt(np.sum(worst*worst)))
 
+    def _init_wave(self, res):
+        self.nominal, self.nominal_focus = float(res.merit[0]), res.focus[0].copy()
+        self.merit_plus, self.merit_minus = res.merit[1::2].copy(), res.merit[2::2].copy()
+        self.focus_plus, self.focus_minus = res.focus[1::2].copy(), res.focus[2::2].copy()
+        self.delta_plus, self.delta_minus = self.merit_plus - self.nominal, self.merit_minus - self.nominal
+        m2 = self.nominal*self.nominal
+        worst = np.maximum(np.maximum(self.merit_plus*self.merit_plus - m2, self.merit_minus*self.merit_minus - m2),
+                           0.0)
+        self.estimated = float(np.sqrt(m2 + np.sum(worst)))
+
 
 class MonteCarlo:
     """Result of ``tolerance_monte_carlo``: ``values`` ``[num_trials, n_tol]`` the drawn changes;
     ``merit`` / ``focus`` ``[num_trials]``; ``nominal``; ``mean``, ``std`` and ``percentiles``
-    {50, 80, 90, 98: M} of the trials' merits; ``result``: the ``TolMerit`` (variant 0 nominal)."""
+    {50, 80, 90, 98: M} of the trials' merits; ``result``: the ``TolMerit`` (variant 0 nominal).  With
+    the wavefront criterion ``result`` is a ``WaveMerit`` and ``focus`` its per-tile ``focus``
+    coefficients ``[num_trials, n_fields, n_wvls]``."""
 
     def __init__(self, tolerances, values, res):
         self.tolerances, self.values, self.result = list(tolerances), values, res
@@ -1684,8 +1742,67 @@ def _tol_records(opt_model, change_sets, num_rays, fields, wvls, foc, table, dev
     return rec.reshape(len(change_sets), len(fields), len(wvls), -1), wvl_wts, field_wts
 
 
+def _tol_wave_records(opt_model, change_sets, num_rays, fields, wvls, foc, table, device, backend, trace_kwargs):
+    """``[n_var, n_fields, n_wvls, RT_WFE_DOUBLES]`` wavefront-error records of every change set on the grid
+    of ``wavefront_error`` (each field's ``RayGrid`` samples, no vignetting, each wavelength referred to
+    its own chief ray), each variant's wave records built on the device; the chief rays' status
+    ``[n_var, n_fields, n_wvls]``, the wavelengths in system units and the spectral / field weights"""
+    from . import tolerance as TOL
+    from .table import describe_model
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    fields = list(osp.field_of_view.fields if fields is None else fields)
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    foc = osp.defocus.focus_shift if foc is None else foc
+    region = osp.spectral_region
+    wvl_wts = [region.spectral_wts[list(region.wavelengths).index(w)] for w in wvls]
+    field_wts = [f.wt for f in fields]
+    descs, n_by_wvl, all_wvls = describe_model(sm)
+    var = [TOL.perturbed_descriptors(descs, n_by_wvl, ch, sm) for ch in change_sets]
+    nb = np.stack([v[1] for v in var])
+    fod = opt_model['analysis_results']['parax_data'].fod
+    parax = (fod.exp_dist, abs(fod.n_obj), abs(fod.n_img))       # nominal, as perturbed_model keeps it
+    trace_kwargs.setdefault('check_apertures', True)
+    if backend is not None:
+        args, kw = _wavefront_grid_args(opt_model, None, num_rays, fields, wvls, foc, None, None)
+        spec = E.PupilGridSpec(*args, **kw)
+        wave, _, status = backend.variant_waves([v[0] for v in var], nb, spec, parax)
+        rec = np.asarray(backend.trace_variants_wfe([v[0] for v in var], nb, spec, np.asarray(wave)))
+        status = np.asarray(status)
+    else:
+        tab = _table_for(opt_model, table, device)
+        args, kw = _wavefront_grid_args(opt_model, tab, num_rays, fields, wvls, foc, None, None)
+        dev = torch.device('cuda', tab.device)
+        with torch.cuda.device(dev):
+            grid = E.PupilGrid(*args, device=tab.device, **kw)
+            vs = E.VariantSet([v[0] for v in var], nb, all_wvls, device=tab.device)
+            wave, _, status = vs.wave(grid, parax)
+            rec = E.trace_grid_variants_wfe(vs, grid, wave, **trace_kwargs).cpu().numpy()     # waits
+            status = status.cpu().numpy()
+            vs.close()
+            grid.close()
+    lam = [opt_model.nm_to_sys_units(w) for w in wvls]
+    n, nf, nw = len(change_sets), len(fields), len(wvls)
+    return rec.reshape(n, nf, nw, -1), status.reshape(n, nf, nw), lam, wvl_wts, field_wts
+
+
+def _tol_result(opt_model, tolerances, sets, criterion, num_rays, fields, wvls, foc, compensate_focus, table,
+                device, backend, trace_kwargs):
+    """the TolMerit (spot) or WaveMerit (wavefront) of every change set"""
+    from . import tolerance as TOL
+    for t in tolerances:
+        TOL.check(opt_model.seq_model, t, criterion)
+    if criterion == 'wavefront':
+        TOL.check_wavefront_model(opt_model.seq_model)
+        rec, st, lam, ww, fw = _tol_wave_records(opt_model, sets, num_rays, fields, wvls, foc, table, device,
+                                                 backend, trace_kwargs)
+        return wave_merit(rec, lam, ww, fw, compensate_focus, st)
+    rec, ww, fw = _tol_records(opt_model, sets, num_rays, fields, wvls, foc, table, device, backend, trace_kwargs)
+    return tol_merit(rec, ww, fw, compensate_focus)
+
+
 def tolerance_sensitivity(opt_model, tolerances, num_rays=32, fields=None, wvls=None, foc=None,
-                          compensate_focus=True, table=None, device=0, backend=None, **trace_kwargs):
+                          compensate_focus=True, table=None, device=0, backend=None, criterion='spot',
+                          **trace_kwargs):
     """Change of the spot merit for each tolerance at +delta and -delta, from one grid trace of all
     variants (``rt_trace_grid_variants``; variant 0 nominal, then +delta, -delta per tolerance).
 
@@ -1695,28 +1812,38 @@ def tolerance_sensitivity(opt_model, tolerances, num_rays=32, fields=None, wvls=
     delta* that minimises M, solved in closed form from the device sums (no second trace).  The
     perturbed systems keep the nominal apertures, vignetting and aim (``tolerance.perturbed_model``).
     ``backend``: the CPU test seam, ``backend.trace_variants(descs, n_by_wvl, grid_spec)`` returning
-    the records and ``backend.chief_ref(descs, n_by_wvl, grid_spec, wvl_idx)`` the reference points."""
-    from . import tolerance as TOL
-    for t in tolerances:
-        TOL.check(opt_model.seq_model, t)
+    the records and ``backend.chief_ref(descs, n_by_wvl, grid_spec, wvl_idx)`` the reference points.
+
+    ``criterion='wavefront'``: the merit is the field-weighted RMS over fields of the polychromatic
+    (spectral weights) RMS wavefront error in waves (``wave_merit``), on the grid of ``wavefront_error``
+    (``RayGrid`` samples over each field's vignetting box, no vignetting, apertures checked), each
+    wavelength of each variant referred to that variant's own chief ray and reference sphere, built on
+    the device (``rt_variants_wave``) and traced with the OPD epilogue in one launch per batch
+    (``rt_trace_grid_variants_wfe``).  The focus compensator removes a focus term per (field,
+    wavelength) tile, fitted on {1, x, y, r^2}: each tile is refocused on its own, which is more
+    optimistic than the spot criterion's one common delta*.  Decenters and tilts of interface n_ifc - 2
+    and models whose OPD cannot be evaluated are refused (``tolerance.check``).  ``backend`` then
+    provides ``variant_waves(descs, n_by_wvl, grid_spec, parax)`` -> (wave, ref_img, status) and
+    ``trace_variants_wfe(descs, n_by_wvl, grid_spec, wave)`` -> the records."""
     sets = [[]]
     for t in tolerances:
         sets += [[(t, float(t.delta))], [(t, -float(t.delta))]]
-    rec, ww, fw = _tol_records(opt_model, sets, num_rays, fields, wvls, foc, table, device, backend, trace_kwargs)
-    return Sensitivity(tolerances, tol_merit(rec, ww, fw, compensate_focus))
+    return Sensitivity(tolerances, _tol_result(opt_model, tolerances, sets, criterion, num_rays, fields, wvls, foc,
+                                               compensate_focus, table, device, backend, trace_kwargs))
 
 
 def tolerance_monte_carlo(opt_model, tolerances, num_trials=1000, seed=0, distribution='normal', num_rays=32,
                           fields=None, wvls=None, foc=None, compensate_focus=True, table=None, device=0,
-                          backend=None, **trace_kwargs):
-    """Spot merit of ``num_trials`` randomly built systems: every trial draws every tolerance
-    (``draw_tolerances``), and all trials (with the nominal system as variant 0) are traced over the
-    nominal grid in one launch per batch.  Merit, focus compensation and ``backend`` as
-    ``tolerance_sensitivity``.  The same seed gives the same result."""
+                          backend=None, criterion='spot', **trace_kwargs):
+    """Spot (or, with ``criterion='wavefront'``, RMS wavefront error) merit of ``num_trials`` randomly
+    built systems: every trial draws every tolerance (``draw_tolerances``), and all trials (with the
+    nominal system as variant 0) are traced over the nominal grid in one launch per batch.  Merit,
+    criterion, focus compensation and ``backend`` as ``tolerance_sensitivity``.  The same seed gives
+    the same result."""
     from . import tolerance as TOL
     for t in tolerances:
-        TOL.check(opt_model.seq_model, t)
+        TOL.check(opt_model.seq_model, t, criterion)
     values = draw_tolerances(tolerances, num_trials, seed, distribution)
     sets = [[]] + [list(zip(tolerances, row)) for row in values]
-    rec, ww, fw = _tol_records(opt_model, sets, num_rays, fields, wvls, foc, table, device, backend, trace_kwargs)
-    return MonteCarlo(tolerances, values, tol_merit(rec, ww, fw, compensate_focus))
+    return MonteCarlo(tolerances, values, _tol_result(opt_model, tolerances, sets, criterion, num_rays, fields, wvls,
+                                                      foc, compensate_focus, table, device, backend, trace_kwargs))

@@ -22,6 +22,10 @@
  *                               reference spheres (rt_refocus.cuh)
  *   k_trace_grid_variants       the whole grid traced once per perturbed prescription of a
  *                               variant set, per-item records (rt_tol.cuh); k_reduce_tol
+ *   k_variants_wave             the chief ray and wave record of every (variant, tile), one thread
+ *                               each (rt_tolwave.cuh)
+ *   k_trace_grid_variants_wfe   k_trace_grid_variants with the OPD epilogue against each variant's
+ *                               wave records, per-item wavefront-error records; k_reduce_variants_wfe
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
  * The surface table (n_ifc x rt_surface_desc + n_wvl x n_ifc indices) is staged
@@ -47,6 +51,7 @@
 #include "rt_mtf.cuh"
 #include "rt_refocus.cuh"
 #include "rt_tol.cuh"
+#include "rt_tolwave.cuh"
 
 using namespace b200rt;
 
@@ -143,6 +148,7 @@ struct rt_variants {
     unsigned long long *d_counters;     /* ring of RT_COUNTERS work counters */
     void *d_block;
     std::atomic<unsigned> next_counter;
+    std::vector<unsigned char> wave_ok; /* [n_var] rt_table::wave_ok of each variant */
 };
 
 /* what the grid kernel needs, passed by value */
@@ -529,11 +535,51 @@ struct RefocusPlanes {
     int32_t n, pad_;
 };
 
-/* the perturbed prescriptions of one rt_trace_grid_variants launch */
+/* the perturbed prescriptions of one rt_trace_grid_variants[_wfe] launch */
 struct VariantPlan {
-    double *items;              /* DEVICE [n_var][n_tiles][chunks_per_tile*RT_WARPS][RT_TOL_DOUBLES] */
-    int32_t n_var, pad_;
+    double *items;              /* DEVICE [n_var][n_tiles][chunks_per_tile*RT_WARPS][RT_TOL_DOUBLES] (WFE:
+                                 * [RT_WFE_DOUBLES]) */
+    int32_t n_var, n_tiles;
+    const double *wave;         /* WFE: DEVICE [n_var][n_tiles][RT_WAVE_DOUBLES] */
 };
+
+/* one work item of the variants wavefront-error trace: its whole RT_WFE_DOUBLES record (every
+ * column written, so scratch needs no clearing) -- the 13 sums by wfe_item_sums_store's halving
+ * tree, the counts by ballots, min / max W, the valid flag.  reduce_tile<WfeLayout> then adds a
+ * (variant, tile)'s items in item order, as k_reduce_wfe adds rt_trace_grid_wfe's item sums. */
+__device__ __forceinline__ void wfe_var_item(bool have, int status, double W, double x, double y,
+                                             double *__restrict__ dst)
+{
+    const int lane = threadIdx.x & 31;
+    const bool ok = have && status == RT_RAY_OK;
+    wfe_item_sums_store(ok, W, x, y, dst + 7);
+    const int ck = status == RT_RAY_OK ? 0 : (status <= RT_RAY_BLOCKED ? status : 4);
+    double cnt = 0.0;
+#pragma unroll
+    for (int c = 0; c < 5; c++) {
+        const unsigned m = __ballot_sync(0xffffffffu, have && ck == c);
+        if (lane == 2*c + 1) cnt = (double)__popc(m);
+    }
+    /* min / max as wfe_item: the lower half-warp reduces min, the upper max; lanes 0 and 16 */
+    const bool h16 = lane & 16;
+    const double mn = ok ? W : CUDART_INF, mx = ok ? W : -CUDART_INF;
+    const double got = __shfl_xor_sync(0xffffffffu, h16 ? mn : mx, 16);
+    double b = h16 ? fmax(mx, got) : fmin(mn, got);
+#pragma unroll
+    for (int s = 8; s > 0; s >>= 1) {
+        const double o = __shfl_xor_sync(0xffffffffu, b, s);
+        b = h16 ? fmax(b, o) : fmin(b, o);
+    }
+    /* odd lanes 1..9: counts 0..4 (the even lanes < 26 hold the sums); 0 / 16: min / max;
+     * 11: valid flag; 13, 15, 17: the zero columns 21-23 */
+    if ((lane & 1) && lane <= 9) dst[lane >> 1] = cnt;
+    if (lane == 0) dst[5] = b;
+    if (lane == 16) dst[6] = b;
+    if (lane == 11) dst[20] = 1.0;
+    if (lane == 13) dst[21] = 0.0;
+    if (lane == 15) dst[22] = 0.0;
+    if (lane == 17) dst[23] = 0.0;
+}
 
 /* chunk loop shared by the general and the lean grid kernels: start ray ->
  * trace -> per-ray results -> transverse aberration (focus_pupil_coords,
@@ -542,7 +588,9 @@ struct VariantPlan {
  * (needs WAVE, SUMMARY == false and a work counter).  OPDF: the OPD against every sphere of *RP
  * instead of out.opd (needs WAVE alone).  NRML: see store_result.  VARIANTS: the chunk range once per prescription of *VP,
  * work item u of variant u / (items of the range); trace gets the variant as a seventh argument; no
- * per-ray outputs; the item's tol_item record instead (needs a work counter and nothing else). */
+ * per-ray outputs; the item's tol_item record instead (needs a work counter and nothing else); with
+ * WAVE and WFE the OPD against the variant's own wave record of *VP and the item's wfe_var_item
+ * record instead. */
 template <bool SUMMARY, bool WAVE, bool FOCUS = false, bool NRML = true, bool WFE = false, bool OPDF = false,
           bool VARIANTS = false, typename TraceFn>
 __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_begin, int64_t chunk_end,
@@ -551,7 +599,7 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
                                                 TraceFn trace, const FocusPlanes *FP = nullptr,
                                                 const RefocusPlanes *RP = nullptr, const VariantPlan *VP = nullptr)
 {
-    static_assert(!VARIANTS || (!SUMMARY && !WAVE && !FOCUS && !WFE && !OPDF), "VARIANTS writes its own records");
+    static_assert(!VARIANTS || (!SUMMARY && !FOCUS && !OPDF && WAVE == WFE), "VARIANTS writes its own records");
     static_assert(!WFE || (WAVE && !SUMMARY && !FOCUS), "WFE needs the OPD epilogue and no spot sums");
     static_assert(!OPDF || (WAVE && !SUMMARY && !FOCUS && !WFE), "OPDF needs the OPD epilogue alone");
     const int64_t tile0 = chunk_begin/G.chunks_per_tile;
@@ -624,16 +672,18 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
                     for (int pl = 0; pl < RP->n; pl++) dst[pl*RP->n_rays] = CUDART_NAN;
                 }
             } else if (WAVE) {
+                const double *wr = VARIANTS ? VP->wave + ((int64_t)var*VP->n_tiles + tile)*RT_WAVE_DOUBLES
+                                            : G.wave + tile*RT_WAVE_DOUBLES;
                 const double opd = (R.status == RT_RAY_OK)
-                                       ? wave_opd(G.wave + tile*RT_WAVE_DOUBLES, R.p1, d0, R.pk, R.dk, R.p, R.d, R.op)
+                                       ? wave_opd(wr, R.p1, d0, R.pk, R.dk, R.p, R.d, R.op)
                                        : CUDART_NAN;
-                if (!WFE || out.opd) out.opd[k] = opd;
+                if (!VARIANTS && (!WFE || out.opd)) out.opd[k] = opd;
                 if (WFE) {
                     wW = opd;
                     grid_pupil_coords(G, f, loc, wx, wy);
                 }
             }
-            if (VARIANTS || out.abr_x || SUMMARY) {
+            if ((VARIANTS && !WFE) || out.abr_x || SUMMARY) {
                 const double rx = G.ref_img ? G.ref_img[tile*2 + 0] : 0.0;
                 const double ry = G.ref_img ? G.ref_img[tile*2 + 1] : 0.0;
                 double dist = div_maybe_zero(G.foc, R.d.z);
@@ -665,13 +715,14 @@ __device__ __forceinline__ void grid_chunk_loop(const GridDev &G, int64_t chunk_
             focus_item(*FP, have, status, fp, fd, op, (int)(tile/G.n_wvls), tile, lc, slice, item, chunk_slots,
                        first, sl, scratch, item_sums);
         }
-        if (WFE) {
+        if (WFE && !VARIANTS) {
             const bool first = tile != cur_tile;
             cur_tile = tile;
             wfe_item(have, status, wW, wx, wy, tile, first, sl, scratch, item_sums + item*RT_WFE_ITEM_SUMS);
         }
         /* a variant's items are its tiles' items in order: item u is record u */
-        if (VARIANTS) tol_item(have, status, ax, ay, op, fd, VP->items + item*RT_TOL_DOUBLES);
+        if (VARIANTS && !WFE) tol_item(have, status, ax, ay, op, fd, VP->items + item*RT_TOL_DOUBLES);
+        if (VARIANTS && WFE) wfe_var_item(have, status, wW, wx, wy, VP->items + item*RT_WFE_DOUBLES);
         if (!work_counter) c += gridDim.x;
     }
     if (SUMMARY && !chunk_slots && cur_tile >= 0) acc_flush(acc, scratch, cur_tile, blockIdx.x, sl);
@@ -792,6 +843,52 @@ k_trace_grid_variants(const rt_surface_desc *__restrict__ g_surfs, const double 
             trace_ray<false, false>(g_surfs + (int64_t)v*n_ifc, g_n + ((int64_t)v*n_wvl + wi)*n_ifc, g_wvl[wi],
                                     n_ifc, o, p0, d0, fw, R);
         }, nullptr, nullptr, &P);
+}
+
+/* k_trace_grid_variants with the OPD epilogue (rt_trace_grid_variants_wfe): each ray's OPD against
+ * its variant's wave record of P.wave, per-item wavefront-error records */
+__global__ void __launch_bounds__(RT_BLOCK)
+k_trace_grid_variants_wfe(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                          int n_ifc, int n_wvl, GridDev G, int64_t n_chunks, rt_opts o,
+                          const double *__restrict__ g_wvl, int pupil_kind, unsigned long long *work_counter,
+                          VariantPlan P)
+{
+    const rt_out out = {};
+    grid_chunk_loop<false, true, false, false, true, false, true>(G, 0, n_chunks, out, nullptr, nullptr,
+                                                                  work_counter, nullptr,
+        [&](int f, int w, int64_t loc, int64_t k, RayResult &R, Vec3 &d0, int v) {
+            Vec3 p0;
+            grid_start_ray<false>(G, pupil_kind, f, loc, p0, d0);
+            FullWriter fw = {nullptr, 0};
+            const int wi = G.wvl_idx[w];
+            trace_ray<false, true>(g_surfs + (int64_t)v*n_ifc, g_n + ((int64_t)v*n_wvl + wi)*n_ifc, g_wvl[wi],
+                                   n_ifc, o, p0, d0, fw, R);
+        }, nullptr, nullptr, &P);
+}
+
+/* the wave record of every (variant, tile) of rt_variants_wave, one thread each: the chief ray of
+ * k_chief_ref (pupil (0, 0), no vignetting) at the tile's wavelength through the variant's rows,
+ * then tolwave_record.  g_surfs / g_n: the set's rows from the launch's first variant on */
+__global__ void k_variants_wave(const rt_surface_desc *__restrict__ g_surfs, const double *__restrict__ g_n,
+                                int n_ifc, int n_wvl, GridDev G, int n_tiles, int n_var, int pupil_kind,
+                                const double *__restrict__ g_wvl, rt_opts o, double exp_dist, double n_obj,
+                                double n_img, double *__restrict__ wave, double *__restrict__ ref_img,
+                                int32_t *__restrict__ status)
+{
+    const int64_t i = (int64_t)blockIdx.x*blockDim.x + threadIdx.x;
+    if (i >= (int64_t)n_var*n_tiles) return;
+    const int v = (int)(i/n_tiles), tile = (int)(i - (int64_t)v*n_tiles);
+    const int f = tile/G.n_wvls, w = tile - f*G.n_wvls;
+    const rt_surface_desc *tab = g_surfs + (int64_t)v*n_ifc;
+    const int wi = G.wvl_idx[w];
+    Vec3 p0, d0;
+    grid_start_ray_at<false>(G, pupil_kind, f, 0.0, 0.0, false, p0, d0);
+    FullWriter fw = {nullptr, 0};
+    RayResult R;
+    trace_ray<false, true>(tab, g_n + ((int64_t)v*n_wvl + wi)*n_ifc, g_wvl[wi], n_ifc, o, p0, d0, fw, R);
+    tolwave_record(R.status, R.p1, d0, R.pk, R.dk, R.p, R.d, R.op, G.foc, tab[n_ifc - 2], exp_dist, n_obj, n_img,
+                   wave + i*RT_WAVE_DOUBLES, ref_img + i*2);
+    status[i] = R.status;
 }
 
 /* ---- lean kernels: plan built in shared memory by the CTA (rt_lean.cuh) */
@@ -1145,6 +1242,14 @@ k_reduce_tol(const double *__restrict__ items, int64_t items_per_tile, double *p
              double *__restrict__ record)
 {
     reduce_tile<TolLayout, false>(items, items_per_tile, partials, tickets, record, nullptr, 0, 0, 1, 0, 0);
+}
+
+/* k_reduce_tol for the per-item wavefront-error records of rt_trace_grid_variants_wfe */
+__global__ void __launch_bounds__(RT_RED_THREADS)
+k_reduce_variants_wfe(const double *__restrict__ items, int64_t items_per_tile, double *partials,
+                      unsigned int *tickets, double *__restrict__ record)
+{
+    reduce_tile<WfeLayout, false>(items, items_per_tile, partials, tickets, record, nullptr, 0, 0, 1, 0, 0);
 }
 
 /* summary of an empty chunk range: zero counts / sums, identities in the min / max columns */
@@ -1764,6 +1869,72 @@ static int check_descs(const char *fn, const rt_surface_desc *surfs, int64_t n)
         if (s.n_phase_coefs < 0 || s.n_phase_coefs > RT_MAX_PHASE_COEFS)
             return fail(RT_ERR_INVALID, "%s: phase coefficient count out of range", fn);
     }
+    return RT_OK;
+}
+
+/* RT_ERR_UNSUPPORTED unless every variant of [var_begin, var_end) can carry the OPD epilogue (the
+ * refusal of rt_trace_grid_wfe: >= 3 interfaces and no decenter on the last one before the image --
+ * which also keeps the image gap of an infinite-reference tile untilted and undecentered) */
+static int check_variants_wave(const char *fn, const rt_variants *v, int32_t var_begin, int32_t var_end)
+{
+    for (int32_t i = var_begin; i < var_end; i++)
+        if (!v->wave_ok[i])
+            return fail(RT_ERR_UNSUPPORTED, "%s: opd needs >= 3 interfaces and no decenter on the last one before "
+                        "the image", fn);
+    return RT_OK;
+}
+
+/* rt_trace_grid_variants[_wfe]: the argument checks, the scratch (item records | partials | tickets; both
+ * records are 24 doubles) and the two launches.  wfe: the _wfe launch, whose wave records are `wave` */
+template <typename Kern, typename Red>
+static int variants_launch(const char *fn, Kern kern, Red red, bool wfe, const rt_variants *v, const rt_grid *g,
+                           int32_t var_begin, int32_t var_end, const rt_opts *o, const double *wave, double *record,
+                           void *scratch, void *stream)
+{
+    static_assert(RT_TOL_DOUBLES == RT_WFE_DOUBLES, "one scratch layout");
+    if (!v || !g || !o) return fail(RT_ERR_INVALID, "%s: bad arguments", fn);
+    if (var_begin < 0 || var_end > v->n_var || var_end < var_begin)
+        return fail(RT_ERR_INVALID, "%s: variant range out of bounds", fn);
+    if (var_end > var_begin && (!record || !scratch))
+        return fail(RT_ERR_INVALID, "%s: record and scratch are required", fn);
+    if (wfe && var_end > var_begin && !wave) return fail(RT_ERR_INVALID, "%s: wave records are required", fn);
+    if (v->device != g->device)
+        return fail(RT_ERR_INVALID, "%s: variants and grid on different devices", fn);
+    if (o->wvl_idx < 0 || o->wvl_idx >= v->n_wvl) return fail(RT_ERR_INVALID, "opts.wvl_idx out of range");
+    for (int32_t wi : g->h_wvl_idx)
+        if (wi < 0 || wi >= v->n_wvl)
+            return fail(RT_ERR_INVALID, "%s: the grid's wvl_idx is out of range for the variants", fn);
+    if (wfe)
+        if (int rc = check_variants_wave(fn, v, var_begin, var_end)) return rc;
+    if (var_end == var_begin) return RT_OK;
+    DeviceGuard guard(v->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const int32_t n_var = var_end - var_begin;
+    const int64_t tiles = (int64_t)n_var*g->n_tiles;
+    const int64_t n_items = n_var*g->n_chunks*RT_WARPS;
+    double *items = (double *)scratch;
+    double *partials = items + n_items*RT_TOL_DOUBLES;
+    unsigned int *tickets = (unsigned int *)(partials + tiles*RT_RED_SPLIT*RT_TOL_DOUBLES);
+    /* every item record is written by the trace and every partial before it is read: clear the tickets */
+    CUDA_TRY(cudaMemsetAsync(tickets, 0, (size_t)tiles*sizeof(unsigned int), s));
+    rt_variants *vv = const_cast<rt_variants *>(v);
+    unsigned long long *wc = v->d_counters + (vv->next_counter++ % RT_COUNTERS);
+    CUDA_TRY(cudaMemsetAsync(wc, 0, sizeof(unsigned long long), s));
+    VariantPlan P;
+    P.items = items; P.n_var = n_var; P.n_tiles = (int32_t)g->n_tiles; P.wave = wave;
+    int grid;
+    int rc = persistent_grid(kern, 0, v->sm_count, n_items/RT_WARPS, &grid);
+    if (rc) return rc;
+    kern<<<grid, RT_BLOCK, 0, s>>>(v->d_surfs + (int64_t)var_begin*v->n_ifc,
+                                   v->d_n + (int64_t)var_begin*v->n_wvl*v->n_ifc, v->n_ifc,
+                                   v->n_wvl, grid_dev(g), g->n_chunks, *o, v->d_wvl,
+                                   g->pupil_kind, wc, P);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    red<<<(unsigned)(tiles*RT_RED_SPLIT), RT_RED_THREADS, 0, s>>>(
+        items, g->chunks_per_tile*RT_WARPS, partials, tickets, record);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
     return RT_OK;
 }
 
@@ -2499,6 +2670,11 @@ int rt_variants_create(const rt_surface_desc *surfs, int32_t n_ifc, const double
     if (!v) return fail(RT_ERR_NOMEM, "rt_variants_create: out of host memory");
     v->device = device; v->n_ifc = n_ifc; v->n_wvl = n_wvl; v->n_var = n_var;
     v->sm_count = prop.multiProcessorCount;
+    v->wave_ok.resize((size_t)n_var);
+    for (int32_t i = 0; i < n_var; i++) {      /* as rt_table_create's wave_ok */
+        const rt_surface_desc &k = surfs[(int64_t)i*n_ifc + n_ifc - 2];
+        v->wave_ok[i] = n_ifc >= 3 && k.has_tfrm == 0 && k.t[0] == 0.0 && k.t[1] == 0.0;
+    }
     v->d_block = nullptr; v->next_counter = 0;
     cudaError_t e = cudaMalloc(&v->d_block, h.size() + b_c);
     if (e == cudaSuccess) e = cudaMemcpy(v->d_block, h.data(), h.size(), cudaMemcpyHostToDevice);
@@ -2540,43 +2716,50 @@ int64_t rt_grid_variants_scratch_bytes(const rt_grid *g, int32_t n_var)
 int rt_trace_grid_variants(const rt_variants *v, const rt_grid *g, int32_t var_begin, int32_t var_end,
                            const rt_opts *o, double *record, void *scratch, void *stream)
 {
-    if (!v || !g || !o) return fail(RT_ERR_INVALID, "rt_trace_grid_variants: bad arguments");
+    return variants_launch("rt_trace_grid_variants", k_trace_grid_variants, k_reduce_tol, false, v, g, var_begin,
+                           var_end, o, nullptr, record, scratch, stream);
+}
+
+int64_t rt_grid_variants_wfe_scratch_bytes(const rt_grid *g, int32_t n_var)
+{
+    return rt_grid_variants_scratch_bytes(g, n_var);      /* the same layout: RT_WFE_DOUBLES == RT_TOL_DOUBLES */
+}
+
+int rt_trace_grid_variants_wfe(const rt_variants *v, const rt_grid *g, int32_t var_begin, int32_t var_end,
+                               const rt_opts *o, const double *wave, double *record, void *scratch, void *stream)
+{
+    return variants_launch("rt_trace_grid_variants_wfe", k_trace_grid_variants_wfe, k_reduce_variants_wfe, true, v, g,
+                           var_begin, var_end, o, wave, record, scratch, stream);
+}
+
+int rt_variants_wave(const rt_variants *v, const rt_grid *g, int32_t var_begin, int32_t var_end, const double *parax,
+                     double *wave, double *ref_img, int32_t *status, void *stream)
+{
+    if (!v || !g) return fail(RT_ERR_INVALID, "rt_variants_wave: bad arguments");
     if (var_begin < 0 || var_end > v->n_var || var_end < var_begin)
-        return fail(RT_ERR_INVALID, "rt_trace_grid_variants: variant range out of bounds");
-    if (var_end > var_begin && (!record || !scratch))
-        return fail(RT_ERR_INVALID, "rt_trace_grid_variants: record and scratch are required");
+        return fail(RT_ERR_INVALID, "rt_variants_wave: variant range out of bounds");
+    if (var_end > var_begin && (!parax || !wave || !ref_img || !status))
+        return fail(RT_ERR_INVALID, "rt_variants_wave: parax, wave, ref_img and status are required");
     if (v->device != g->device)
-        return fail(RT_ERR_INVALID, "rt_trace_grid_variants: variants and grid on different devices");
-    if (o->wvl_idx < 0 || o->wvl_idx >= v->n_wvl) return fail(RT_ERR_INVALID, "opts.wvl_idx out of range");
+        return fail(RT_ERR_INVALID, "rt_variants_wave: variants and grid on different devices");
     for (int32_t wi : g->h_wvl_idx)
         if (wi < 0 || wi >= v->n_wvl)
-            return fail(RT_ERR_INVALID, "rt_trace_grid_variants: the grid's wvl_idx is out of range for the variants");
+            return fail(RT_ERR_INVALID, "rt_variants_wave: the grid's wvl_idx is out of range for the variants");
+    if (int rc = check_variants_wave("rt_variants_wave", v, var_begin, var_end)) return rc;
     if (var_end == var_begin) return RT_OK;
     DeviceGuard guard(v->device);
-    cudaStream_t s = (cudaStream_t)stream;
+    /* the chief-ray options of waveabr.trace_chief_rays: trace_grid's defaults, apertures not checked */
+    rt_opts o;
+    o.eps = 1.0e-12; o.pt_inside_fuzz = -1.0;
+    o.check_apertures = 0; o.intersect_obj = g->pupil_kind == RT_PUPIL_WIDE ? 0 : 1;
+    o.filter_out_phantoms = 0; o.first_surf = 1; o.last_surf = v->n_ifc - 2; o.wvl_idx = 0;
     const int32_t n_var = var_end - var_begin;
-    const int64_t tiles = (int64_t)n_var*g->n_tiles;
-    double *items = (double *)scratch;
-    double *partials = items + tol_items(g, n_var)*RT_TOL_DOUBLES;
-    unsigned int *tickets = (unsigned int *)(partials + tiles*RT_RED_SPLIT*RT_TOL_DOUBLES);
-    /* every item record is written by the trace and every partial before it is read: clear the tickets */
-    CUDA_TRY(cudaMemsetAsync(tickets, 0, (size_t)tiles*sizeof(unsigned int), s));
-    rt_variants *vv = const_cast<rt_variants *>(v);
-    unsigned long long *wc = v->d_counters + (vv->next_counter++ % RT_COUNTERS);
-    CUDA_TRY(cudaMemsetAsync(wc, 0, sizeof(unsigned long long), s));
-    VariantPlan P;
-    P.items = items; P.n_var = n_var; P.pad_ = 0;
-    int grid;
-    int rc = persistent_grid(k_trace_grid_variants, 0, v->sm_count, tol_items(g, n_var)/RT_WARPS, &grid);
-    if (rc) return rc;
-    k_trace_grid_variants<<<grid, RT_BLOCK, 0, s>>>(v->d_surfs + (int64_t)var_begin*v->n_ifc,
-                                                    v->d_n + (int64_t)var_begin*v->n_wvl*v->n_ifc, v->n_ifc,
-                                                    v->n_wvl, grid_dev(g), g->n_chunks, *o, v->d_wvl,
-                                                    g->pupil_kind, wc, P);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    k_reduce_tol<<<(unsigned)(tiles*RT_RED_SPLIT), RT_RED_THREADS, 0, s>>>(
-        items, g->chunks_per_tile*RT_WARPS, partials, tickets, record);
+    const int64_t n = (int64_t)n_var*g->n_tiles;
+    const int threads = 128;
+    k_variants_wave<<<(unsigned)((n + threads - 1)/threads), threads, 0, (cudaStream_t)stream>>>(
+        v->d_surfs + (int64_t)var_begin*v->n_ifc, v->d_n + (int64_t)var_begin*v->n_wvl*v->n_ifc, v->n_ifc, v->n_wvl,
+        grid_dev(g), (int)g->n_tiles, n_var, g->pupil_kind, v->d_wvl, o, parax[0], parax[1], parax[2], wave, ref_img,
+        status);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RT_OK;

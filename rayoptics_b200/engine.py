@@ -21,7 +21,7 @@ import torch
 from . import _abi
 from ._abi import (rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES, RT_WFE_DOUBLES,
                    RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS, RT_MTF_DOUBLES, RT_MTF_MAX_RAYS, RT_SPHERE_DOUBLES,
-                   RT_TOL_DOUBLES)
+                   RT_TOL_DOUBLES, RT_WAVE_DOUBLES)
 
 SUMMARY_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other',
                   'sum_x', 'sum_y', 'sum_xx', 'sum_yy', 'sum_xy',
@@ -1040,6 +1040,27 @@ class VariantSet:
             raise RuntimeError('VariantSet was destroyed')
         return self._handle
 
+    def wave(self, grid, parax, var_begin=0, var_end=None):
+        """The wave records of variants ``[var_begin, var_end)`` on every tile of ``grid``, built on the
+        device (``rt_variants_wave``): each variant's chief rays, reference spheres at ``grid.foc`` and
+        ``waveabr.wave_record``.  ``parax``: the nominal ``(fod.exp_dist, |fod.n_obj|, |fod.n_img|)``.
+        Returns ``(wave [n, n_tiles, RT_WAVE_DOUBLES], ref_img [n, n_tiles, 2], status [n, n_tiles])``
+        device tensors; a tile whose chief ray does not reach the image has status != 0 and a NaN
+        record.  Asynchronous on the current CUDA stream."""
+        device = torch.device('cuda', self.device)
+        var_end = self.n_var if var_end is None else int(var_end)
+        n = max(var_end - int(var_begin), 0)
+        wave = torch.empty((n, grid.n_tiles, RT_WAVE_DOUBLES), dtype=torch.float64, device=device)
+        ref = torch.empty((n, grid.n_tiles, 2), dtype=torch.float64, device=device)
+        status = torch.empty((n, grid.n_tiles), dtype=torch.int32, device=device)
+        px = np.ascontiguousarray(parax, dtype=np.float64)
+        if px.shape != (3,):
+            raise ValueError('parax must be (exp_dist, |n_obj|, |n_img|)')
+        _abi.check(self._lib.rt_variants_wave(self.handle, grid.handle, int(var_begin), var_end,
+                                              px.ctypes.data_as(_abi.c_double_p), _ptr(wave), _ptr(ref),
+                                              _ptr(status), _stream_ptr(device)))
+        return wave, ref, status
+
     def close(self):
         if getattr(self, '_handle', None) is not None:
             self._lib.rt_variants_destroy(self._handle)
@@ -1085,6 +1106,43 @@ def trace_grid_variants(variants, grid, var_begin=0, var_end=None, cap=VARIANT_S
         v1 = min(v0 + batch, var_end)
         _abi.check(lib.rt_trace_grid_variants(variants.handle, grid.handle, v0, v1, C.byref(opts),
                                               _ptr(rec[v0 - var_begin]), _ptr(scratch), stream))
+    rec._keep = scratch            # scratch must outlive the asynchronous launches
+    return rec
+
+
+def trace_grid_variants_wfe(variants, grid, wave, var_begin=0, var_end=None, cap=VARIANT_SCRATCH_CAP, **kwargs):
+    """Wavefront-error records of variants ``[var_begin, var_end)`` of a VariantSet over the whole
+    PupilGrid (``rt_trace_grid_variants_wfe``): ``[n, n_tiles, RT_WFE_DOUBLES]`` float64 device tensor
+    (WFE_FIELDS; ``wavefront_statistics`` turns it into numbers), each ray's OPD referred to its
+    variant's record of ``wave`` ``[n, n_tiles, RT_WAVE_DOUBLES]`` (``VariantSet.wave`` of the same
+    range).  Batches, trace defaults and stream as ``trace_grid_variants``."""
+    lib = _abi.load_library()
+    device = torch.device('cuda', variants.device)
+    var_end = variants.n_var if var_end is None else int(var_end)
+    kwargs.setdefault('check_apertures', True)
+    kwargs.setdefault('first_surf', 1)
+    kwargs.setdefault('last_surf', variants.n_ifc - 2)
+    if grid.pupil_kind == _abi.PUPIL_WIDE:
+        kwargs['intersect_obj'] = False
+    opts = _abi.make_opts(**kwargs)
+    n = max(var_end - int(var_begin), 0)
+    rec = torch.empty((n, grid.n_tiles, RT_WFE_DOUBLES), dtype=torch.float64, device=device)
+    if n == 0:
+        return rec
+    if tuple(wave.shape) != (n, grid.n_tiles, RT_WAVE_DOUBLES) or wave.dtype != torch.float64 \
+            or wave.device != device or not wave.is_contiguous():
+        raise ValueError('wave must be a contiguous float64 [n, n_tiles, RT_WAVE_DOUBLES] tensor on the '
+                         'variants\' device')
+    per = max(1, int(lib.rt_grid_variants_wfe_scratch_bytes(grid.handle, 1)))
+    batch = max(1, min(n, cap//per))
+    scratch = torch.empty(max(int(lib.rt_grid_variants_wfe_scratch_bytes(grid.handle, batch))//8, 1),
+                          dtype=torch.float64, device=device)
+    stream = _stream_ptr(device)
+    for v0 in range(int(var_begin), var_end, batch):
+        v1 = min(v0 + batch, var_end)
+        i = v0 - int(var_begin)
+        _abi.check(lib.rt_trace_grid_variants_wfe(variants.handle, grid.handle, v0, v1, C.byref(opts),
+                                                  _ptr(wave[i]), _ptr(rec[i]), _ptr(scratch), stream))
     rec._keep = scratch            # scratch must outlive the asynchronous launches
     return rec
 

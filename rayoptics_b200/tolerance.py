@@ -48,8 +48,23 @@ class Tolerance:
     delta: float
 
 
-def check(sm, tol):
-    """ValueError unless ``tol`` can be applied to the sequential model ``sm``"""
+def check_wavefront_model(sm):
+    """ValueError unless the OPD of the sequential model ``sm`` can be evaluated (``wavefront_error``):
+    at least 3 interfaces and no decenter or tilt on interface n_ifc - 2, the last before the image"""
+    if len(sm.ifcs) < 3:
+        raise ValueError('the wavefront criterion needs at least 3 interfaces')
+    rt, t = sm.lcl_tfrms[-2]
+    if not np.array_equal(rt, np.identity(3)) or t[0] != 0.0 or t[1] != 0.0:
+        raise ValueError('the wavefront criterion needs an image gap without decenter or tilt on interface '
+                         f'{len(sm.ifcs) - 2}, the last before the image')
+
+
+def check(sm, tol, criterion='spot'):
+    """ValueError unless ``tol`` can be applied to the sequential model ``sm``.  ``criterion='wavefront'``
+    also refuses models whose OPD cannot be evaluated (``check_wavefront_model``) and decenters / tilts
+    of interface n_ifc - 2, which would tilt the image gap"""
+    if criterion not in ('spot', 'wavefront'):
+        raise ValueError(f'unknown criterion {criterion!r}')
     n_ifc = len(sm.ifcs)
     if tol.kind not in KINDS:
         raise ValueError(f'unknown tolerance kind {tol.kind!r}')
@@ -67,6 +82,11 @@ def check(sm, tol):
             raise ValueError(f'radius tolerance on the plane interface {i}')
     if (tol.kind == 'thickness' or tol.kind in _DECENTER_KINDS) and sm._tfrms_given is not None:
         raise ValueError(f'{tol.kind} tolerance on a model whose transforms were given explicitly')
+    if criterion == 'wavefront':
+        check_wavefront_model(sm)
+        if tol.kind in _DECENTER_KINDS and i == n_ifc - 2:
+            raise ValueError(f'{tol.kind} tolerance on interface {i}, the last before the image: the wavefront '
+                             'criterion needs an image gap without decenter or tilt')
 
 
 def _new_profile(prof, kind, d):
