@@ -50,6 +50,8 @@ extern "C" {
 #define RT_MTF_DOUBLES 8     /* per-tile record of rt_grid_mtf */
 #define RT_SPHERE_DOUBLES 8  /* per-(plane, tile) reference-sphere record of rt_trace_grid_opd_focus */
 #define RT_TOL_DOUBLES 24    /* per-(variant, tile) record of rt_trace_grid_variants */
+#define RT_ILLUM_DOUBLES 10  /* per-tile record of rt_grid_illumination */
+#define RT_ILLUM_MAX_RAYS 1024 /* pupil samples per side of rt_grid_illumination */
 
 /* error codes (function return values) */
 enum rt_error {
@@ -563,6 +565,26 @@ int64_t rt_grid_variants_wfe_scratch_bytes(const rt_grid *grid, int32_t n_var);
 int rt_trace_grid_variants_wfe(const rt_variants *variants, const rt_grid *grid, int32_t var_begin,
                                int32_t var_end, const rt_opts *opts, const double *wave, double *record,
                                void *scratch, void *stream);
+
+/* ---- relative illumination (ABI 6, additive): the image-space projected solid angle of every tile
+ * of a grid trace, Omega = integral of |d(L, M)/d(x, y)| over the unit pupil disk (csrc/rt_illum.cuh;
+ * DESIGN.md section 4).  The grid must be a product grid (paired = 0) without apply_vignetting with
+ * nx = ny = n, 2 <= n <= RT_ILLUM_MAX_RAYS.  status, dx, dy: DEVICE per-ray outputs of an rt_trace_grid
+ * over all chunks (dx, dy: direction cosines L, M of the last segment); ray (i, j) of tile t is entry
+ * t*n*n + i*n + j, at relative pupil coordinates (x, y) = (pupil_x[i], pupil_y[j]) of its field.
+ * A ray is used when its status is 0 and x*x + y*y <= 1.  For F in {L, M} its derivative along x is
+ * central (F[i+1] - F[i-1])/(x[i+1] - x[i-1]) when rays i-1 and i+1 of its column both have status 0,
+ * else forward (F[i+1] - F[i])/(x[i+1] - x[i]) when ray i+1 has, else backward (F[i] - F[i-1])/(x[i] -
+ * x[i-1]) when ray i-1 has, else it is not formed; the same along y (index j).  J = Lx*My - Ly*Mx with
+ * every product rounded once.  A used ray with a derivative not formed is isolated and adds nothing.
+ * record: DEVICE [n_tiles][RT_ILLUM_DOUBLES]:
+ *   0-4 status-class counts of every ray (as the wavefront-error record)   5 n_used
+ *   6 n_disk (grid points with x*x + y*y <= 1, any status)   7 n_isolated   8 sum |J|   9 sum J
+ * Sum order: each column j added along i in increasing i from +0.0, the column sums added in
+ * increasing j from +0.0.  Bit-reproducible, independent of the launch shape.  RT_ERR_INVALID before
+ * any device work for a bad grid or a NULL pointer.  One launch on `stream`. */
+int rt_grid_illumination(const rt_grid *grid, const int32_t *status, const double *dx, const double *dy,
+                         double *record, void *stream);
 
 /* ---- misc */
 const char *rt_last_error(void);

@@ -24,6 +24,8 @@ RT_MTF_MAX_RAYS = 1024
 RT_MTF_DOUBLES = 8
 RT_SPHERE_DOUBLES = 8
 RT_TOL_DOUBLES = 24
+RT_ILLUM_DOUBLES = 10
+RT_ILLUM_MAX_RAYS = 1024
 
 # enum rt_profile
 PROFILE_IDS = {'Spherical': 0, 'Conic': 1, 'EvenPolynomial': 2,
@@ -131,7 +133,8 @@ EXPORTS = ['rt_table_create', 'rt_table_destroy', 'rt_table_dims', 'rt_table_set
            'rt_grid_zernike_scratch_bytes', 'rt_grid_zernike', 'rt_combine_zernike', 'rt_grid_aim_chief',
            'rt_grid_pupil_function', 'rt_grid_mtf', 'rt_grid_mtf_shifts', 'rt_trace_grid_opd_focus',
            'rt_variants_create', 'rt_variants_destroy', 'rt_grid_variants_scratch_bytes', 'rt_trace_grid_variants',
-           'rt_variants_wave', 'rt_grid_variants_wfe_scratch_bytes', 'rt_trace_grid_variants_wfe']
+           'rt_variants_wave', 'rt_grid_variants_wfe_scratch_bytes', 'rt_trace_grid_variants_wfe',
+           'rt_grid_illumination']
 
 _lib = None
 
@@ -230,6 +233,8 @@ def load_library():
     lib.rt_grid_variants_wfe_scratch_bytes.restype = i64
     lib.rt_trace_grid_variants_wfe.argtypes = [vp, vp, i32, i32, C.POINTER(rt_opts), vp, vp, vp, vp]
     lib.rt_trace_grid_variants_wfe.restype = i32
+    lib.rt_grid_illumination.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.rt_grid_illumination.restype = i32
     lib.rt_last_error.restype = C.c_char_p
     lib.rt_abi_version.restype = i32
     lib.rt_chunk_rays.restype = i32

@@ -994,6 +994,137 @@ def field_map(opt_model, num_fields=9, num_rays=32, num_terms=37, wvls=None, foc
                     zernike=zf, wvls=wvls, num_rays=num_rays, num_terms=num_terms)
 
 
+class RelativeIllumination:
+    """Result of ``relative_illumination``, per field and wavelength (``[n_fields, n_wvls]`` arrays).
+
+    ``omega``: the projected solid angle of the image-space beam (steradians of direction-cosine area,
+    in the image interface's frame); ``ri``: omega over the reference field's at the same wavelength;
+    ``f_number``: the effective F-number 1/(2 |n'| sqrt(omega/pi)); ``fold``: 1 - |sum J|/sum |J|, nonzero
+    where the pupil-to-direction map folds over; ``n_used``, ``n_disk``, ``n_isolated`` and the ray
+    counts ``n_ok``, ``n_missed``, ``n_tir``, ``n_blocked``, ``n_other``; ``cra``: the chief ray's angle
+    to the image interface's axis in degrees; ``chief_img`` ``[..., 2]`` and ``chief_dir`` ``[..., 3]``:
+    its image point and last direction (NaN where the chief ray does not reach the image).
+    ``ri_poly`` ``[n_fields]``: the spectrally weighted ratio with weights ``wts``; ``n_img`` ``[n_wvls]``:
+    |n'|; ``fields``: the traced fields, ``ref_index``: the reference field's index among them;
+    ``record``: the ``[n_tiles, RT_ILLUM_DOUBLES]`` device records."""
+
+    def __init__(self, **kw):
+        for k, v in kw.items():
+            setattr(self, k, v)
+
+
+def _illumination_host(spec, status, d):
+    """The ``[n_tiles, RT_ILLUM_DOUBLES]`` records of traced rays, formed on the host (the ``backend=``
+    test seam; the device forms them in ``rt_grid_illumination``)"""
+    n, per = spec.nx, spec.rays_per_tile
+    rec = np.zeros((spec.n_tiles, E.RT_ILLUM_DOUBLES))
+    for t in range(spec.n_tiles):
+        f = t//spec.n_wvls
+        sl = slice(t*per, (t + 1)*per)
+        rec[t] = E.illumination_sums_host(status[sl].reshape(n, n), d[0, sl].reshape(n, n),
+                                          d[1, sl].reshape(n, n), spec.pupil_x[f], spec.pupil_y[f])
+    return rec
+
+
+def _aim(opt_model, fields, tab, device, backend):
+    from . import vigcalc as V
+    cwl = opt_model.optical_spec.spectral_region.central_wvl
+    if backend is not None:
+        backend.aim_fields(opt_model, fields, cwl)
+    else:
+        V.aim_fields_on_device(opt_model, fields, cwl, table=tab, device=device)
+
+
+def relative_illumination(opt_model, num_rays=128, fields=None, wvls=None, num_fields=None, table=None, device=0,
+                          backend=None, **trace_kwargs):
+    """Relative illumination, effective F-number and chief-ray angle of every field and wavelength, from
+    one grid trace.
+
+    For a Lambertian object the image irradiance is proportional to the projected solid angle omega =
+    integral of dL dM over the image-space beam (L, M: direction cosines in the image interface's frame),
+    vignetting by the real apertures, pupil aberration and obliquity included, transmission left out.
+    Each tile is a ``num_rays`` x ``num_rays`` grid over relative pupil [-1, 1]^2
+    (``engine.accumulated_steps``), aimed at the field's aim point, no vignetting factors applied,
+    apertures checked; omega = pi sum |J|/n_disk with J the Jacobian d(L, M)/d(x, y) of the used rays
+    (``rt_grid_illumination``, DESIGN.md section 4).  RI is omega over the reference field's at the same
+    wavelength; the reference field is the first field at (0, 0), or an axial field added to ``fields``
+    and aimed like ``field_map``'s points.
+
+    ``fields``: default the model's own; ``num_fields=K`` instead traces K points at relative field y =
+    ``linspace(0, 1, K)``, scaled and aimed on the device as ``field_map``'s (not for wide-angle fields
+    or angular pupils: NotImplementedError).  ``num_rays``: 2 ... RT_ILLUM_MAX_RAYS.  ``backend``: the
+    CPU test seam -- ``backend.chief_rays`` as ``zernike_fit``'s, ``backend.aim_fields`` as
+    ``field_map``'s, and ``backend.trace_directions(opt_model, spec, check_apertures)`` -> ``{'status',
+    'd'}``.  ``trace_kwargs``: trace options (default ``check_apertures=True``).  Launches: the chief
+    rays, the trace and the sums (plus the aiming of added fields).  Returns a
+    ``RelativeIllumination``."""
+    n = int(num_rays)
+    if not 2 <= n <= E.RT_ILLUM_MAX_RAYS:
+        raise ValueError(f'num_rays must be 2 ... {E.RT_ILLUM_MAX_RAYS}')
+    osp, sm = opt_model.optical_spec, opt_model.seq_model
+    fov = osp.field_of_view
+    tab = None if backend is not None else _table_for(opt_model, table, device)
+    if num_fields is not None:
+        if fields is not None:
+            raise ValueError('give fields or num_fields, not both')
+        k = int(num_fields)
+        if k < 1:
+            raise ValueError('num_fields must be at least 1')
+        scale = fov.max_field()[0]
+        if fov.is_relative and fov.value != 0:
+            scale = scale/fov.value
+        fields = [Field(x=0.0, y=float(scale*r), fov=fov) for r in np.linspace(0.0, 1.0, k)]
+        _aim(opt_model, fields, tab, device, backend)
+    fields = list(fov.fields if fields is None else fields)
+    ref = next((i for i, f in enumerate(fields) if f.x == 0 and f.y == 0), None)
+    if ref is None:
+        axial = Field(fov=fov)
+        try:
+            _aim(opt_model, [axial], tab, device, backend)
+        except NotImplementedError as e:
+            raise ValueError('relative_illumination: this model\'s fields cannot be aimed on the device; '
+                             'pass fields= including an axial field (x = y = 0)') from e
+        fields.append(axial)
+        ref = len(fields) - 1
+    wvls = list(sm.wvlns if wvls is None else wvls)
+    nf, nw = len(fields), len(wvls)
+    trace_kwargs.setdefault('check_apertures', True)
+    full, _, cstatus = (W.trace_chief_rays(opt_model, tab, fields, wvls) if backend is None
+                        else backend.chief_rays(opt_model, fields, wvls))
+    wvl_index = sm.index_for_wavelength if tab is None else tab.wvl_index
+    args, kw = E._grid_args(opt_model, wvl_index, n, fields, wvls, None, (-1.0, 1.0), False)
+    if backend is not None:
+        spec = E.PupilGridSpec(*args, **kw)
+        r = backend.trace_directions(opt_model, spec, trace_kwargs['check_apertures'])
+        rec = _illumination_host(spec, np.asarray(r['status']), np.asarray(r['d']))
+    else:
+        dev = torch.device('cuda', tab.device)
+        with torch.cuda.device(dev):
+            grid = E.PupilGrid(*args, device=tab.device, **kw)
+            rec = E.trace_grid_illumination(tab, grid, **trace_kwargs).cpu().numpy()   # one small copy; waits
+            grid.close()
+    shape = (nf, nw)
+    out = {k: rec[:, i].reshape(shape) for i, k in enumerate(E.ILLUM_RECORD[:8])}
+    with np.errstate(invalid='ignore', divide='ignore'):
+        omega = (np.pi*rec[:, 8]/rec[:, 6]).reshape(shape)
+        ri = omega/omega[ref]
+        fold = (1.0 - np.abs(rec[:, 9])/rec[:, 8]).reshape(shape)
+        n_img = np.array([abs(sm.gaps[-1].medium.rindex(w)) for w in wvls])
+        f_number = 1.0/(2.0*n_img*np.sqrt(omega/np.pi))
+        region = osp.spectral_region
+        wts = np.array([region.spectral_wts[list(region.wavelengths).index(w)] for w in wvls], dtype=np.float64)
+        ri_poly = (omega @ wts)/(omega[ref] @ wts)
+    last = np.asarray(full)[-1]                                   # [10, n_tiles]: the image segment
+    ok = (np.asarray(cstatus).reshape(-1) == 0)[:, None]
+    chief_img = np.where(ok, last[0:2].T, np.nan).reshape(nf, nw, 2)
+    chief_dir = np.where(ok, last[3:6].T, np.nan).reshape(nf, nw, 3)
+    cra = np.degrees(np.arctan2(np.hypot(chief_dir[..., 0], chief_dir[..., 1]), np.abs(chief_dir[..., 2])))
+    out.update(omega=omega, ri=ri, f_number=f_number, fold=fold, ri_poly=ri_poly, wts=wts, n_img=n_img,
+               cra=cra, chief_img=chief_img, chief_dir=chief_dir, record=rec, fields=fields, ref_index=ref,
+               wvls=wvls, num_rays=n)
+    return RelativeIllumination(**out)
+
+
 # --------------------------------------------------------------------------
 # RayFan / RayList / RayGrid: the reference's analysis classes
 # (/root/reference/src/rayoptics/raytr/analyses.py:121-187,343-434,584-663) with

@@ -26,6 +26,8 @@
  *                               each (rt_tolwave.cuh)
  *   k_trace_grid_variants_wfe   k_trace_grid_variants with the OPD epilogue against each variant's
  *                               wave records, per-item wavefront-error records; k_reduce_variants_wfe
+ *   k_illumination              projected solid angle of every tile from a grid trace's per-ray
+ *                               status and last directions, one CTA cluster per tile (rt_illum.cuh)
  *   k_dfma_peak                 fp64 FMA microbenchmark (roofline denominator)
  *
  * The surface table (n_ifc x rt_surface_desc + n_wvl x n_ifc indices) is staged
@@ -52,6 +54,10 @@
 #include "rt_refocus.cuh"
 #include "rt_tol.cuh"
 #include "rt_tolwave.cuh"
+#include "rt_illum.cuh"
+#include <cooperative_groups.h>
+
+namespace cg = cooperative_groups;
 
 using namespace b200rt;
 
@@ -1547,6 +1553,144 @@ k_mtf(GridDev G, const int32_t *__restrict__ status, const MtfC *__restrict__ P,
     }
 }
 
+/* ---- relative illumination (rt_grid_illumination; rt_illum.cuh).  Tiles of n x n rays, ray (i, j) at
+ * i*n + j.  A tile's columns are split over a cluster of RT_ILLUM_CLUSTER_MAX CTAs at most, one thread per
+ * column. */
+#define RT_ILLUM_THREADS 128
+#define RT_ILLUM_CLUSTER_MAX 8
+
+/* one row of a column as a thread walks it: its pupil x, and status, L, M (status -1 past the grid's
+ * edge); the lanes at a warp's edge also hold the ray beside them in the next warp's column (e*) */
+struct IllumRow {
+    int st, est;
+    double x, L, M, eL, eM;
+};
+
+/* row i of the column that starts at ray `col` */
+__device__ __forceinline__ IllumRow illum_row(const int32_t *__restrict__ status, const double *__restrict__ L,
+                                              const double *__restrict__ M, const double *__restrict__ px,
+                                              int64_t col, int n, int i, bool in, int de, bool edge)
+{
+    IllumRow w{-1, -1, 0.0, 0.0, 0.0, 0.0, 0.0};
+    if (i < n) {
+        const int64_t r = col + (int64_t)i*n;
+        w.x = px[i];
+        if (in) {
+            w.st = status[r];
+            w.L = L[r];
+            w.M = M[r];
+        }
+        if (in && edge) {
+            w.est = status[r + de];
+            w.eL = L[r + de];
+            w.eM = M[r + de];
+        }
+    }
+    return w;
+}
+
+__device__ __forceinline__ IllumPt illum_pt(int st, double L, double M)
+{
+    return IllumPt{L, M, st == 0};
+}
+
+/* One cluster of CTAs per tile; CTA `rank` of the cluster takes columns rank*blockDim.x ..., one thread
+ * per column.  Each thread walks its column in increasing i with rows i-1, i, i+1 in registers and rows
+ * i+2, i+3 already loaded, so a warp's loads are 32 adjacent rays of one row; the neighbours along j come
+ * from the adjacent lanes (the lanes at a warp's edge load theirs with the row).  The column chains and
+ * the counts go to the shared memory of the cluster's first CTA, whose thread 0 adds the columns in
+ * increasing j (rt_illum.cuh).  No atomics, no scratch. */
+__global__ void __launch_bounds__(RT_ILLUM_THREADS)
+k_illumination(GridDev G, const int32_t *__restrict__ status, const double *__restrict__ L,
+               const double *__restrict__ M, double *__restrict__ rec)
+{
+    __shared__ double col_abs[RT_ILLUM_MAX_RAYS], col_j[RT_ILLUM_MAX_RAYS];
+    __shared__ int cnt[RT_ILLUM_CLUSTER_MAX*RT_ILLUM_THREADS/32][8];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int rank = (int)cluster.block_rank(), n_cta = (int)cluster.num_blocks();
+    const int n = G.nx;
+    const int64_t tile = blockIdx.x/n_cta;
+    const int f = (int)(tile/G.n_wvls);
+    const double *px = G.pupil_x + (int64_t)f*n, *py = G.pupil_y + (int64_t)f*n;
+    const int lane = threadIdx.x & 31, de = lane == 0 ? -1 : 1;
+    const int j = rank*blockDim.x + threadIdx.x;
+    const bool in = j < n;
+    const bool edge = (lane == 0 && j > 0) || (lane == 31 && j + 1 < n);
+    const double y0 = in ? py[j] : 0.0;
+    const double y_m = in && j > 0 ? py[j - 1] : y0, y_p = in && j + 1 < n ? py[j + 1] : y0;
+    const int64_t col = tile*G.rays_per_tile + j;
+    int c[8] = {0, 0, 0, 0, 0, 0, 0, 0};       /* status classes 0-4, used, disk, isolated */
+    IllumRow r0{-1, -1, 0.0, 0.0, 0.0, 0.0, 0.0};
+    IllumRow r1 = illum_row(status, L, M, px, col, n, 0, in, de, edge);
+    IllumRow r2 = illum_row(status, L, M, px, col, n, 1, in, de, edge);
+    IllumRow r3 = illum_row(status, L, M, px, col, n, 2, in, de, edge);
+    IllumRow r4 = illum_row(status, L, M, px, col, n, 3, in, de, edge);
+    IllumAcc acc{0.0, 0.0};
+    /* unrolled by the window's length, so that the rows rotate by renaming: a copy would wait for the
+     * load of row i+4 one iteration after it was issued */
+#pragma unroll 5
+    for (int i = 0; i < n; i++) {
+        /* row i's neighbours along j */
+        int st_m = __shfl_up_sync(0xffffffffu, r1.st, 1), st_p = __shfl_down_sync(0xffffffffu, r1.st, 1);
+        double L_m = __shfl_up_sync(0xffffffffu, r1.L, 1), L_p = __shfl_down_sync(0xffffffffu, r1.L, 1);
+        double M_m = __shfl_up_sync(0xffffffffu, r1.M, 1), M_p = __shfl_down_sync(0xffffffffu, r1.M, 1);
+        if (lane == 0) {
+            st_m = r1.est;
+            L_m = r1.eL;
+            M_m = r1.eM;
+        }
+        if (lane == 31) {
+            st_p = r1.est;
+            L_p = r1.eL;
+            M_p = r1.eM;
+        }
+        const double x0 = r1.x, x_m = i > 0 ? r0.x : x0, x_p = i + 1 < n ? r2.x : x0;
+        if (in) {
+            const int ck = (r1.st >= 0 && r1.st <= RT_RAY_BLOCKED) ? r1.st : 4;
+#pragma unroll
+            for (int q = 0; q < 5; q++) c[q] += ck == q;          /* constant indices: c stays in registers */
+            c[6] += x0*x0 + y0*y0 <= 1.0;
+            if (illum_used(r1.st, x0, y0)) {
+                c[5]++;
+                if (!illum_term(acc, illum_pt(r1.st, r1.L, r1.M), illum_pt(r0.st, r0.L, r0.M),
+                                illum_pt(r2.st, r2.L, r2.M), illum_pt(st_m, L_m, M_m), illum_pt(st_p, L_p, M_p),
+                                x_m, x0, x_p, y_m, y0, y_p))
+                    c[7]++;
+            }
+        }
+        r0 = r1;
+        r1 = r2;
+        r2 = r3;
+        r3 = r4;
+        r4 = illum_row(status, L, M, px, col, n, i + 4, in, de, edge);
+    }
+#pragma unroll
+    for (int q = 0; q < 8; q++) c[q] = __reduce_add_sync(0xffffffffu, c[q]);
+    cluster.sync();                                     /* every CTA of the cluster has started */
+    double *abs0 = cluster.map_shared_rank(col_abs, 0), *j0 = cluster.map_shared_rank(col_j, 0);
+    int *cnt0 = cluster.map_shared_rank(&cnt[0][0], 0);
+    if (in) {
+        abs0[j] = acc.abs_j;
+        j0[j] = acc.j;
+    }
+    if (lane == 0) {
+        const int w = rank*(int)(blockDim.x/32) + (int)(threadIdx.x/32);
+#pragma unroll
+        for (int q = 0; q < 8; q++) cnt0[w*8 + q] = c[q];
+    }
+    cluster.sync();
+    if (rank == 0 && threadIdx.x == 0) {
+        for (int w = 1; w < n_cta*(int)(blockDim.x/32); w++)
+#pragma unroll
+            for (int q = 0; q < 8; q++) c[q] += cnt[w][q];
+        double *out = rec + tile*RT_ILLUM_DOUBLES;
+#pragma unroll
+        for (int q = 0; q < 8; q++) out[q] = (double)c[q];
+        out[8] = illum_line_sum(col_abs, n);
+        out[9] = illum_line_sum(col_j, n);
+    }
+}
+
 /* chief rays of all fields: pupil (0, 0), no vignetting, apertures not checked, general
  * per-ray code on the global table (bit-identical to the lean loop by construction, and
  * n_fields rays do not need the specialised kernel).  One thread per field. */
@@ -2904,6 +3048,41 @@ int rt_grid_mtf_shifts(const rt_grid *g, const int32_t *status, const double *pu
     if (n_shifts > 0 && (!shifts || !acf_x || !acf_y))
         return fail(RT_ERR_INVALID, "rt_grid_mtf_shifts: shifts, acf_x and acf_y are required when n_shifts > 0");
     return launch_mtf(g, status, pupil, pupil_t, shifts, n_shifts, acf_x, acf_y, record, stream);
+}
+
+int rt_grid_illumination(const rt_grid *g, const int32_t *status, const double *dx, const double *dy,
+                         double *record, void *stream)
+{
+    const char *fn = "rt_grid_illumination";
+    if (!g) return fail(RT_ERR_INVALID, "%s: grid is required", fn);
+    if (g->paired) return fail(RT_ERR_INVALID, "%s: needs a product grid (paired = 0)", fn);
+    if (g->apply_vignetting)
+        return fail(RT_ERR_INVALID, "%s: the pupil coordinates must not be vignetted (apply_vignetting = 0)", fn);
+    if (g->nx != g->ny) return fail(RT_ERR_INVALID, "%s: needs a square grid (nx = ny)", fn);
+    if (g->nx < 2 || g->nx > RT_ILLUM_MAX_RAYS)
+        return fail(RT_ERR_INVALID, "%s: nx must lie in 2 ... RT_ILLUM_MAX_RAYS", fn);
+    if (!status || !dx || !dy || !record)
+        return fail(RT_ERR_INVALID, "%s: status, dx, dy and record are required", fn);
+    DeviceGuard guard(g->device);
+    const int n = g->nx;
+    /* at most RT_ILLUM_THREADS columns per CTA, whole warps: n <= 1024 needs at most 8 CTAs */
+    const int n_cta = (n + RT_ILLUM_THREADS - 1)/RT_ILLUM_THREADS;
+    const int threads = ((n + n_cta - 1)/n_cta + 31)/32*32;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(g->n_tiles*n_cta));
+    cfg.blockDim = dim3((unsigned)threads);
+    cfg.stream = (cudaStream_t)stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)n_cta;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, k_illumination, grid_dev(g), status, dx, dy, record));
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RT_OK;
 }
 
 /* fp64 vector-pipe peak, measured with a DFMA chain kernel: the roofline

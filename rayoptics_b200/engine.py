@@ -21,7 +21,7 @@ import torch
 from . import _abi
 from ._abi import (rt_out, rt_grid_spec, rt_field_desc, RT_SEG_DOUBLES, RT_SUMMARY_DOUBLES, RT_WFE_DOUBLES,
                    RT_ZERN_DOUBLES, RT_ZERN_MAX_TERMS, RT_MTF_DOUBLES, RT_MTF_MAX_RAYS, RT_SPHERE_DOUBLES,
-                   RT_TOL_DOUBLES, RT_WAVE_DOUBLES)
+                   RT_TOL_DOUBLES, RT_WAVE_DOUBLES, RT_ILLUM_DOUBLES, RT_ILLUM_MAX_RAYS)
 
 SUMMARY_FIELDS = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other',
                   'sum_x', 'sum_y', 'sum_xx', 'sum_yy', 'sum_xy',
@@ -979,6 +979,92 @@ def mtf_sums_host(P):
     s_lines = _line_sums_in_order(P.real) + 1j*_line_sums_in_order(P.imag)       # line j: along i
     S = complex(_line_sums_in_order(s_lines.real[:, None])[0], _line_sums_in_order(s_lines.imag[:, None])[0])
     return _autocorr_host(P), _autocorr_host(P.T), S
+
+
+# --- relative illumination (rt_grid_illumination; the sums of csrc/rt_illum.cuh) ---------------------
+ILLUM_RECORD = ('n_ok', 'n_missed', 'n_tir', 'n_blocked', 'n_other', 'n_used', 'n_disk', 'n_isolated',
+                'sum_abs_j', 'sum_j')
+
+
+def grid_illumination(grid, status, dx, dy):
+    """``rt_grid_illumination``: the ``[n_tiles, RT_ILLUM_DOUBLES]`` float64 device record
+    (``ILLUM_RECORD``: status counts, n_used, n_disk, n_isolated, sum |J|, sum J) of the projected
+    solid angle of every tile of a square product PupilGrid without vignetting, 2 <= n <=
+    RT_ILLUM_MAX_RAYS.  ``status`` (int32), ``dx``, ``dy`` (float64, the last segment's direction
+    cosines L, M): per-ray device tensors of a grid trace over all chunks.  Asynchronous on the current
+    CUDA stream."""
+    lib = _abi.load_library()
+    _ray_tensor(status, torch.int32, grid.n_rays, 'status')
+    _ray_tensor(dx, torch.float64, grid.n_rays, 'dx')
+    _ray_tensor(dy, torch.float64, grid.n_rays, 'dy')
+    device = status.device
+    rec = torch.empty((grid.n_tiles, RT_ILLUM_DOUBLES), dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        _abi.check(lib.rt_grid_illumination(grid.handle, _ptr(status), _ptr(dx), _ptr(dy), _ptr(rec),
+                                            _stream_ptr(device)))
+    rec._keep = (status, dx, dy)               # must outlive the asynchronous launch
+    return rec
+
+
+def trace_grid_illumination(table, grid, res=None, **kwargs):
+    """The ``grid_illumination`` record of every tile of a square PupilGrid without vignetting:
+    ``trace_grid`` over all chunks with the ``d`` and ``status`` outputs into device buffers (``res``: an
+    optional BundleResult with both, which keeps them), then ``grid_illumination`` -- two launches.
+    Trace defaults as ``trace_grid``."""
+    if res is None:
+        res = BundleResult(grid.n_rays, table.n_ifc, torch.device('cuda', table.device), ('d', 'status'))
+    elif res.d is None or res.status is None:
+        raise ValueError('res needs the d and status outputs')
+    trace_grid(table, grid, 0, grid.n_chunks, summary=False, res=res, **kwargs)
+    rec = grid_illumination(grid, res.status, res.d[0], res.d[1])
+    rec._keep = (rec._keep, res)
+    return rec
+
+
+def _illum_deriv(ok, L, M, u):
+    """``(dL, dM, kind)`` along axis 0 of ``[n, n]`` arrays (``u``: the coordinates of the rows) in the
+    order of rt_illum.cuh's illum_deriv: kind 0 central, 1 forward, 2 backward, 3 not formed"""
+    ok_m, ok_p = np.zeros_like(ok), np.zeros_like(ok)
+    ok_m[1:], ok_p[:-1] = ok[:-1], ok[1:]
+    u0 = u[:, None]
+    u_m, u_p = np.concatenate([u[:1], u[:-1]])[:, None], np.concatenate([u[1:], u[-1:]])[:, None]
+    kind = np.where(ok_m & ok_p, 0, np.where(ok_p, 1, np.where(ok_m, 2, 3)))
+    out = []
+    with np.errstate(invalid='ignore', divide='ignore', over='ignore'):
+        for f in (L, M):
+            f_m, f_p = f.copy(), f.copy()
+            f_m[1:], f_p[:-1] = f[:-1], f[1:]
+            out.append(np.select([kind == 0, kind == 1, kind == 2],
+                                 [(f_p - f_m)/(u_p - u_m), (f_p - f)/(u_p - u0), (f - f_m)/(u0 - u_m)], 0.0))
+    return out[0], out[1], kind
+
+
+def illumination_sums_host(status, L, M, x, y):
+    """The ``RT_ILLUM_DOUBLES`` record of one tile, bit for bit in the order of ``rt_grid_illumination``
+    (the ``backend=`` seam of ``analyses.relative_illumination``).  ``status``, ``L``, ``M``: ``[n, n]``
+    per-ray status and last-segment direction cosines, ray (i, j) at pupil (``x[i]``, ``y[j]``)."""
+    st = np.asarray(status).reshape(len(x), len(y))
+    L = np.asarray(L, dtype=np.float64).reshape(st.shape)
+    M = np.asarray(M, dtype=np.float64).reshape(st.shape)
+    x, y = np.asarray(x, dtype=np.float64), np.asarray(y, dtype=np.float64)
+    ok = st == 0
+    disk = x[:, None]*x[:, None] + y[None, :]*y[None, :] <= 1.0
+    used = ok & disk
+    Lx, Mx, kx = _illum_deriv(ok, L, M, x)
+    Ly, My, ky = (a.T for a in _illum_deriv(ok.T, L.T, M.T, y))
+    formed = used & (kx != 3) & (ky != 3)
+    with np.errstate(invalid='ignore', over='ignore'):
+        a, b = Lx*My, Ly*Mx
+        J = np.where(formed, a - b, 0.0)
+    cols_abs = _line_sums_in_order(np.abs(J))           # column j: along i, increasing i, from +0.0
+    cols_j = _line_sums_in_order(J)
+    rec = np.zeros(RT_ILLUM_DOUBLES)
+    cls = np.where((st >= 0) & (st <= 3), st, 4).ravel()
+    rec[0:5] = np.bincount(cls, minlength=5)[:5]
+    rec[5], rec[6], rec[7] = used.sum(), disk.sum(), (used & ~formed).sum()
+    rec[8] = _line_sums_in_order(cols_abs[:, None])[0]
+    rec[9] = _line_sums_in_order(cols_j[:, None])[0]
+    return rec
 
 
 def measure_fp64_peak(device=0):
